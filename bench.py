@@ -1,12 +1,12 @@
 #!/usr/bin/env python
-"""bench.py -- audio-hours/sec of the inaSpeechSegmenter hot path on B200.
+"""bench.py -- audio-hours/sec of the inaSpeechSegmenter hot path on H100.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--dump-outputs DIR]
 
 One step = one pass of the whole hot path (K1 log-mel/energy -> energy Viterbi
 -> smn CNN -> Viterbi -> gender CNN -> Viterbi -> segment list on the host) over
 one batch of synthetic 16 kHz mono int16 audio: BASELINE.json configs[1]
-("smn+gender on 10 h synthetic, 1xB200").  With N > 1 ranks (torchrun) ONE recording
+("smn+gender on 10 h synthetic", one GPU).  With N > 1 ranks (torchrun) ONE recording
 of N x 10 h is time-sharded over the ranks (inaspeechsegmenter_b200/shard.py:
 34-frame halo, NCCL all-gathers of loge and of the CNN posteriors, BASELINE
 configs[4]) => weak scaling (per-GPU work fixed); the timed region is bracketed
@@ -63,6 +63,8 @@ def parse():
     ap.add_argument('--k1-hours', type=float, default=100.0, help='BASELINE configs[2] size')
     ap.add_argument('--vbx-hours', type=float, default=50.0, help='BASELINE configs[3] size (1 h files)')
     ap.add_argument('--vbx-max-sec', type=float, default=60.0, help='stop the VBx leg after this many seconds (bounded sample)')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write what the last timed step computed (segment list, seeded sample of the CNN posteriors) as DIR/<name>.npy')
     return ap.parse_args()
 
 
@@ -430,7 +432,7 @@ def config2_block(torch, args, dev, peaks, fft):
     L = loge.numel()
     bytes_alg = 420.0 * L                                                # SURVEY 8(d): 320 B int16 in + 100 B out per frame
     gbs = bytes_alg / (ms_k1 * 1e-3) / 1e9
-    peak_gbs = peaks.get('hbm_gbs') or 6650.0
+    peak_gbs = peaks.get('hbm_gbs') or 3350.0
     del mspec, loge
     # ---- the whole sm+gender pass, device-resident and from pinned host memory
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -449,14 +451,14 @@ def config2_block(torch, args, dev, peaks, fft):
     e1.record(); e1.synchronize()
     ms_e2e = e0.elapsed_time(e1)
     out = {
-        'workload': "vad_engine='sm' + gender on %g h synthetic 16 kHz mono int16, 1xB200 (BASELINE configs[2]); one pass each, after a 10-minute warm-up" % hours,
+        'workload': "vad_engine='sm' + gender on %g h synthetic 16 kHz mono int16, one GPU (BASELINE configs[2]); one pass each, after a 10-minute warm-up" % hours,
         'value': hours / (ms_dev * 1e-3), 'unit': UNIT, 'ms': ms_dev,
         'e2e': {'value': hours / (ms_e2e * 1e-3), 'unit': UNIT, 'ms': ms_e2e, 'h2d_bytes': int(n * 2), 'd2h_bytes': int(3 * ((L + 1) // 2)),
                 'equal_to_device_run': bool(segs2 == segs)},
         'segments': len(segs), 'generate_seconds': t_gen,
         'roofline_k1': {'bound': 'hbm', 'kernel': 'sidekit_features_kernel (%s FFT) + loge statistics' % fft, 'achieved': gbs, 'peak': peak_gbs,
                         'unit': 'GB/s', 'frac': gbs / peak_gbs, 'traffic': None,
-                        'peak_source': 'MEASURED_PEAKS.json hbm_gbs (of measured)' if 'hbm_gbs' in peaks else 'fallback 6650 GB/s (of fallback)',
+                        'peak_source': 'MEASURED_PEAKS.json hbm_gbs (of measured)' if 'hbm_gbs' in peaks else 'H100 SXM data sheet, HBM3 3350 GB/s (not measured)',
                         'bytes_per_frame': 420, 'frames': int(L), 'ms': ms_k1, 'launches': int(k1_launches),
                         'x_real_time': hours * 3600 / (ms_k1 * 1e-3)},
     }
@@ -518,7 +520,7 @@ def config3_block(torch, args, dev, peaks):
     ms_e2e = e0.elapsed_time(e1)
     hours = done_files * file_sec / 3600.0
     tf = nwin * ext.flops_per_window / (ms * 1e-3) / 1e12
-    peak_tf = peaks.get('bf16_tflops_sustained') or 1400.0
+    peak_tf = peaks.get('bf16_tflops_sustained') or 989.0
     # CPU: the reference's torch backend (resnet.py, vbx_segmenter.py:271-288) restated, all host cores, a bounded sample of windows
     torch.set_num_threads(host_cores())
     net = vx.ResNet101Oracle(sd)
@@ -552,7 +554,7 @@ def config3_block(torch, args, dev, peaks):
     del keep
     win_per_hour = nwin / hours
     return {
-        'workload': 'VBx x-vector path (features_vbx + resnet.py ResNet101) on %g h synthetic 16 kHz mono as 1 h files, 1xB200 (BASELINE configs[3] = 50 h)' % hours
+        'workload': 'VBx x-vector path (features_vbx + resnet.py ResNet101) on %g h synthetic 16 kHz mono as 1 h files, one GPU (BASELINE configs[3] = 50 h)' % hours
                     + ('' if done_files == nfiles else ' -- BOUNDED SAMPLE: stopped after %g s' % args.vbx_max_sec),
         'value': hours / (ms * 1e-3), 'unit': UNIT, 'ms': ms, 'windows': int(nwin), 'windows_per_s': nwin / (ms * 1e-3),
         'x_real_time': hours * 3600 / (ms * 1e-3), 'gpu_launches': int(launches),
@@ -560,7 +562,7 @@ def config3_block(torch, args, dev, peaks):
                 'h2d_bytes_per_file': int(file_sec * SR * 2), 'd2h_bytes_per_file': int(win_per_hour * 256 * 4)},
         'roofline_k5': {'bound': 'tensor', 'kernel': 'ResNet101 implicit-GEMM convolutions (iss_resnet_embed, 104 conv layers)', 'achieved': tf, 'peak': peak_tf,
                         'unit': 'TFLOP/s', 'frac': tf / peak_tf, 'traffic': None, 'flops_per_window': ext.flops_per_window,
-                        'peak_source': 'MEASURED_PEAKS.json bf16_tflops_sustained (of measured)' if 'bf16_tflops_sustained' in peaks else 'fallback 1.4 PFLOP/s (of fallback)',
+                        'peak_source': 'MEASURED_PEAKS.json bf16_tflops_sustained (of measured)' if 'bf16_tflops_sustained' in peaks else 'H100 SXM data sheet, dense FP16 989 TFLOP/s (not measured)',
                         'note': 'whole x-vector path time (features 0.2 %, ResNet 99 %)'},
         'cpu_baseline': {'value': cpu_win_s / win_per_hour, 'unit': UNIT, 'cores': host_cores(), 'kind': 'port',
                          'sample': '32 windows of 144 frames of the benchmark file through the torch-CPU restatement of resnet.py (the reference\'s own torch backend, vbx_segmenter.py:271-288), all host cores; %.1f windows/s' % cpu_win_s},
@@ -569,7 +571,7 @@ def config3_block(torch, args, dev, peaks):
     }
 
 
-# ----------------------------------------------------------------------------- the B200 arm
+# ----------------------------------------------------------------------------- the GPU arm
 def run_b200(args):
     import ctypes
 
@@ -640,6 +642,8 @@ def run_b200(args):
     ms, segs = timed(step_dev, args.steps)
     launches = lib.iss_launch_count() - l0
     clk = clocks.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, segs, seg if world == 1 else None)
     tms, nlaunch, fl = ctypes.c_double(), ctypes.c_int64(), ctypes.c_double()
     _lib.check(lib.iss_cnn_profile_read(seg.vad.nn.handle, ctypes.byref(tms), ctypes.byref(nlaunch), ctypes.byref(fl)), 'profile_read')
     _lib.check(lib.iss_cnn_profile(seg.vad.nn.handle, -1), 'iss_cnn_profile')
@@ -674,22 +678,21 @@ def run_b200(args):
         peaks = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))
     except Exception:
         pass
-    peak_tf = peaks.get('bf16_tflops_sustained') or 1400.0
-    peak_src = 'MEASURED_PEAKS.json bf16_tflops_sustained (of measured)' if 'bf16_tflops_sustained' in peaks else 'fallback 1.4 PFLOP/s sustained (of fallback)'
+    peak_tf = peaks.get('bf16_tflops_sustained') or 989.0
+    peak_src = 'MEASURED_PEAKS.json bf16_tflops_sustained (of measured)' if 'bf16_tflops_sustained' in peaks else 'H100 SXM data sheet, dense FP16 989 TFLOP/s (not measured)'
     ach = (fl.value / max(nlaunch.value, 1)) / (tms.value / max(nlaunch.value, 1) * 1e-3) / 1e12 if tms.value > 0 else 0.0
     mode = lib.iss_get_gemm_mode()
-    gemm = {0: 'fp32 CUDA cores', 2: 'tcgen05 kind::tf32, 3xTF32 split', 3: 'tcgen05 kind::f16 direct kernel (both operands from shared memory), fp16 hi/lo split (3 products), first layer fused into the operand fill'}.get(mode, 'engine %d' % mode)
-    traffic, traffic_src = ncu_dram_bytes(dominant_profile(mode))
+    gemm = {0: 'fp32 CUDA cores', 2: 'wgmma tf32, 3xTF32 split', 3: 'wgmma f16 (both operands from shared memory), fp16 hi/lo split (3 products), first layer fused into the operand fill'}.get(mode, 'engine %d' % mode)
     roof = {'bound': 'tensor', 'kernel': 'conv_gemm %s (VAD layer %d: %s)' % (gemm, dom, layer_name(seg.vad.nn.lowered.descs[dom])),
-            'achieved': ach, 'peak': peak_tf, 'unit': 'TFLOP/s', 'frac': ach / peak_tf, 'traffic': traffic, 'traffic_source': traffic_src,
+            'achieved': ach, 'peak': peak_tf, 'unit': 'TFLOP/s', 'frac': ach / peak_tf,
             'peak_source': peak_src, 'launches': int(nlaunch.value), 'avg_launch_ms': tms.value / max(nlaunch.value, 1),
             'flops_per_launch': fl.value / max(nlaunch.value, 1), 'share_of_step': tms.value / ms,
-            'note': 'useful fp32-equivalent FLOPs of the layer; the tensor pipe executes 3x as many (hi.hi + hi.lo + lo.hi) on 1/0.773 as many rows (tall-image slots), so the ceiling of this scheme is 0.257; the time includes the fused first layer'}
+            'note': 'useful fp32-equivalent FLOPs of the layer; the tensor pipe executes 3x as many (hi.hi + hi.lo + lo.hi), so the ceiling of this scheme is 1/3; the time includes the fused first layer'}
 
     line = {
         'metric': METRIC, 'value': value, 'unit': UNIT, 'n_gpus': world, 'steps': args.steps, 'warmup': warm,
         'ms_per_step': ms / args.steps, 'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None,
-        'dtype': 'f32' if mode == 0 else ('f32 (3xTF32 split on tcgen05, fp32 accumulate)' if mode == 2 else 'f32 (fp16 hi/lo split on tcgen05 kind::f16, fp32 accumulate; 22 significant bits)'),
+        'dtype': 'f32' if mode == 0 else ('f32 (3xTF32 split on wgmma, fp32 accumulate)' if mode == 2 else 'f32 (fp16 hi/lo split on wgmma f16, fp32 accumulate; 22 significant bits)'),
         'data': 'synthetic',
         'config': {'workload': 'smn+gender on %g h synthetic 16 kHz mono int16 per GPU (BASELINE configs[1])' % args.hours,
                    'networks': 'synthetic-weight stand-ins of the ~1.4M-parameter CNN family (release .hdf5 absent)',
@@ -736,12 +739,6 @@ def run_b200(args):
     return 0
 
 
-def dominant_profile(mode):
-    """The committed `ncu --set full` summary of the dominant kernel for this engine (per-round file name)."""
-    name = {3: 'r02_direct_tc4h_full.txt'}.get(mode)
-    return os.path.join(ROOT, 'profiles', name) if name else None
-
-
 def _strip_cxx_comments(src):
     """C++ source without comments and without white space: the text the compiler's result depends on."""
     out, i, n = [], 0, len(src)
@@ -768,39 +765,36 @@ def kernel_source_hash():
     stamps it into the profile summary."""
     import hashlib
     h = hashlib.sha256()
-    for f in ('conv_gemm_tc_f16d.cu', 'tc_common.cuh', 'conv_gemm.cuh'):
+    for f in ('conv_gemm_tc.cu', 'tc_common.cuh', 'conv_gemm.cuh'):
         with open(os.path.join(ROOT, 'inaspeechsegmenter_b200', 'csrc', f)) as fh:
             h.update(_strip_cxx_comments(fh.read()).encode())
     return h.hexdigest()
 
 
-def ncu_dram_bytes(path):
-    """dram__bytes_read.sum + dram__bytes_write.sum (bytes per launch) of the first kernel in a committed
-    `ncu --set full` summary of the same 8192-patch launch (a profiler cannot run inside the timed process).
-    The summary is stamped with the hash of the kernel sources it was captured from: if they changed since,
-    the figure is withheld (None, 'stale ...') instead of silently going out of date."""
-    if not path or not os.path.exists(path):
-        return None, None
-    try:
-        tot, seen, stamp = 0.0, False, None
-        for line in open(path):
-            if line.startswith('# source_sha256:'):
-                stamp = line.split(':', 1)[1].strip()
-                continue
-            if line.startswith('kernel:'):
-                if seen:
-                    break
-                seen = True
-            elif seen and ('dram__bytes_read.sum ' in line or 'dram__bytes_write.sum ' in line):
-                val, unit = line.split()[-2:]
-                tot += float(val) * {'byte': 1.0, 'Kbyte': 1e3, 'Mbyte': 1e6, 'Gbyte': 1e9}[unit]
-        if stamp != kernel_source_hash():
-            return None, 'stale: %s was captured from other kernel sources' % os.path.relpath(path, ROOT)
-        if tot > 0:
-            return tot, 'ncu --set full, %s (bytes per launch, cold cache; capture of an identical launch, not this run)' % os.path.relpath(path, ROOT)
-    except Exception:
-        pass
-    return None, None
+SEGMENT_LABELS = ('noEnergy', 'speech', 'music', 'noise', 'female', 'male')
+DUMP_PROB_ROWS = 1 << 18
+
+
+def dump_outputs(out_dir, segs, seg):
+    """What the caller of the timed path receives from its last step: the segment list as float64 [n, 3]
+    (label index into SEGMENT_LABELS, start s, stop s), and, on one GPU (seg given), the per-patch softmax of both CNNs
+    (float32; a fixed, seeded sample of DUMP_PROB_ROWS rows when there are more, with the row indices alongside).  A
+    time-sharded run writes the segment list only: each rank holds the posteriors of its own shard."""
+    os.makedirs(out_dir, exist_ok=True)
+    arr = np.array([(SEGMENT_LABELS.index(lab), a, b) for lab, a, b in segs], dtype=np.float64).reshape(-1, 3)
+    np.save(os.path.join(out_dir, 'segments.npy'), arr)
+    if seg is None:
+        return
+    for name, net in (('vad', seg.vad), ('gender', seg.gender)):
+        p = net.last_probs
+        if p is None:
+            continue
+        p = p.float().cpu().numpy() if hasattr(p, 'cpu') else np.asarray(p, dtype=np.float32)
+        rows = np.arange(len(p))
+        if len(p) > DUMP_PROB_ROWS:
+            rows = np.sort(np.random.default_rng(20261015).choice(len(p), DUMP_PROB_ROWS, replace=False))
+        np.save(os.path.join(out_dir, '%s_probs.npy' % name), p[rows].astype(np.float32))
+        np.save(os.path.join(out_dir, '%s_prob_rows.npy' % name), rows.astype(np.float64))
 
 
 def layer_name(d):

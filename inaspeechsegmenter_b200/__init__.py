@@ -1,4 +1,4 @@
-"""inaspeechsegmenter_b200 -- B200-native (sm_100a) implementation of the
+"""inaspeechsegmenter_b200 -- H100-native (sm_90a) implementation of the
 per-frame hot path of ina-foss/inaSpeechSegmenter behind the reference's own
 API (``Segmenter``, ``seg2csv``; inaSpeechSegmenter/__init__.py:26-29).
 

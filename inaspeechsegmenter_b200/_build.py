@@ -1,4 +1,4 @@
-"""In-tree build of libiss_b200.so (sm_100a only) with nvcc.
+"""In-tree build of libiss_b200.so (sm_90a only) with nvcc.
 
 The shared library lives next to this file so that it travels with the source
 tree (it is git-ignored, not pip-installed).  There is deliberately no CPU
@@ -13,7 +13,7 @@ PKG = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG, 'csrc')
 LIB = os.path.join(PKG, 'libiss_b200.so')
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
+FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
          '-Xcompiler', '-fPIC', '-Xptxas', '-v']
 
 
@@ -47,7 +47,7 @@ def build(force=False, verbose=False):
         log.append('== %s\n%s' % (os.path.basename(src), out))
         if p.returncode != 0:
             raise RuntimeError('nvcc failed on %s:\n%s' % (src, out))
-    link = subprocess.run([NVCC, '-shared', '-o', LIB] + objs + ['-lcudart'],
+    link = subprocess.run([NVCC, '-shared', '-gencode', 'arch=compute_90a,code=sm_90a', '-o', LIB] + objs + ['-lcudart'],
                           stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if link.returncode != 0:
         raise RuntimeError('link failed:\n' + link.stdout)

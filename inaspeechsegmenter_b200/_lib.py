@@ -1,7 +1,7 @@
 """ctypes binding of libiss_b200.so (the C ABI declared in include/iss_b200.h).
 
 This is the thin FFI layer the north-star asks for: Python host code calling
-hand-written sm_100a CUDA through a C ABI; torch tensors only supply device
+hand-written sm_90a CUDA through a C ABI; torch tensors only supply device
 memory (``data_ptr()``) and streams.  There is no fallback: if the library is
 missing or a call fails, an exception is raised.
 """
@@ -35,7 +35,7 @@ LAYER_CONV2D, LAYER_DENSE, LAYER_MAXPOOL = 1, 2, 3
 F_BIAS, F_AFFINE_PRE, F_RELU, F_AFFINE_POST, F_SOFTMAX, F_SIGMOID = 1, 2, 4, 8, 16, 32
 PCM_F32, PCM_S16 = 0, 1
 FFT_FP32, FFT_FP64 = 0, 1
-GEMM_FP32, GEMM_TC_TS, GEMM_TC_F16 = 0, 2, 3     # fp32 CUDA cores | 3xTF32 tcgen05 | fp16-split tcgen05 (default)
+GEMM_FP32, GEMM_TC_TS, GEMM_TC_F16 = 0, 2, 3     # fp32 CUDA cores | 3xTF32 wgmma | fp16-split wgmma (default)
 ABI_VERSION = 2                       # == ISS_ABI_VERSION in include/iss_b200.h
 
 # name -> (restype, argtypes); must list every symbol include/iss_b200.h declares

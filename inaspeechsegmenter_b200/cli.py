@@ -25,7 +25,7 @@ def build_parser():
     p = argparse.ArgumentParser(description=description)
     p.add_argument('-i', '--input', nargs='+', required=True, help='Input media to analyse (paths, glob patterns or http urls)')
     p.add_argument('-o', '--output_directory', required=True, help='Directory used to store segmentations')
-    p.add_argument('-s', '--batch_size', type=int, default=32, help='kept for compatibility (the B200 kernels batch internally)')
+    p.add_argument('-s', '--batch_size', type=int, default=32, help='kept for compatibility (the GPU kernels batch internally)')
     p.add_argument('-d', '--vad_engine', choices=['sm', 'smn'], default='smn')
     p.add_argument('-g', '--detect_gender', choices=['true', 'false'], default='True')
     p.add_argument('-b', '--ffmpeg_binary', default='ffmpeg', help='ffmpeg binary; "None" disables ffmpeg (16 kHz WAV input only)')

@@ -130,7 +130,7 @@ struct FirstArgs {
     float *out;
     int64_t n;
     int H, W, OH, OW, KH, KW, SH, SW, PT, PL, Hp, Wp, Cout, flags;
-    int out_packed;        // 1: store split-half words (lo16 << 16 | hi16) for the fp16-split slab convolution behind this layer
+    int out_packed;        // 1: store split-half words (lo16 << 16 | hi16) for the fp16-split convolution behind this layer
 };
 
 constexpr int FIRST_P = 4;
@@ -324,7 +324,7 @@ maxpool_nhwc_vec4_kernel(const float4 *__restrict__ in, float4 *__restrict__ out
     out[i] = best;
 }
 
-// Pooling over split-half words (the tensor between two fp16-split slab convolutions): the window maximum is taken on
+// Pooling over split-half words (the tensor between two fp16-split convolutions): the window maximum is taken on
 // the decoded values hi + lo (exact in fp32) and the winning WORD is stored, so the value itself is unchanged.
 __global__ void __launch_bounds__(256)
 maxpool_nhwc_packed_kernel(const uint4 *__restrict__ in, uint4 *__restrict__ out, int64_t total4, int H, int W, int C4,
@@ -460,7 +460,7 @@ extern "C" int iss_cnn_create(iss_ctx *ctx, const iss_layer_desc *layers, int n_
         if (C % 32 != 0 || K % 32 != 0 || d.cout % 32 != 0) continue;
         int rc = iss_prepare_tc_weights(h_blob + d.w_off, K, d.cout, &L.d_wt, &L.Kp);
         if (rc != ISS_OK) { iss_cnn_destroy(m); return rc; }
-        if (d.cin % 64 == 0) {                                    // fp16-split engine (slab or gather kernel)
+        if (d.cin % 64 == 0) {                                    // fp16-split engine (engine 3)
             rc = iss_prepare_f16_weights(h_blob + d.w_off, K, d.cout, &L.d_wt_f16, &L.f16_inv_scale);
             if (rc != ISS_OK) { iss_cnn_destroy(m); return rc; }
         }
@@ -541,19 +541,15 @@ void fill_conv_args(const Layer &Lr, int64_t nb, ConvArgs &a)
     }
 }
 
-// Will this Conv2D / Dense layer run on the fp16-split engine (slab kernel for un-padded stride-1 KHxKW convolutions,
-// gather kernel for everything else it has a weight image for)?  Only those kernels read / write split-half words.
+// Will this Conv2D / Dense layer run on the fp16-split engine?  Only that engine reads / writes split-half words.
+// ('same' padding with an extra bottom / right row is covered: rows past the input are zero-filled.)
 bool f16_engine_covers(const Layer &L, const ConvArgs &a)
 {
-    if (L.d.kind == ISS_LAYER_MAXPOOL) return false;
-    if (L.d.kind == ISS_LAYER_CONV2D && L.d.pad_bottom == 0 && L.d.pad_right == 0 && iss_conv_f16_slab_covers(a)) return true;
-    // the gather kernel takes symmetric padding only through PT / PL + the bounds check: 'same' padding with an extra
-    // bottom / right row is covered too (rows past the input are zero-filled)
-    return iss_conv_f16_gather_covers(a);
+    return L.d.kind != ISS_LAYER_MAXPOOL && iss_conv_f16_covers(a);
 }
 
 // Should the tensor produced by layer `li` be stored as split-half words?  Yes iff the next compute layer
-// (pooling layers in between keep the format) is a convolution the fp16-split slab kernel takes.
+// (pooling layers in between keep the format) is a convolution the fp16-split engine takes.
 bool wants_packed_output(const iss_cnn *cnn, size_t li, int64_t nb)
 {
     if (iss_get_gemm_mode() != ISS_GEMM_TC_F16) return false;
@@ -647,7 +643,7 @@ extern "C" int iss_cnn_forward(iss_ctx *ctx, iss_cnn *cnn, const float *d_mspec,
         const float *cur = nullptr;
         int which = 0;
         bool cur_packed = false;                                 // format of `cur`: fp32 values or split-half words
-        FirstFuse ffuse = {};                                    // set by layer 0 when it is folded into layer 1's slab fill
+        FirstFuse ffuse = {};                                    // set by layer 0 when it is folded into layer 1's operand fill
         bool first_fused = false;
         int pend_pool_h = 0, pend_pool_w = 0;                    // un-pooled dims of a MaxPooling2D folded into the next convolution
         for (size_t li = 0; li < cnn->layers.size(); ++li) {
@@ -667,8 +663,8 @@ extern "C" int iss_cnn_forward(iss_ctx *ctx, iss_cnn *cnn, const float *d_mspec,
                 ISS_CUDA_OK(cudaEventRecord(cnn->prof_ev[cnn->prof_used], st));
             }
             if (d.kind == ISS_LAYER_MAXPOOL && cur_packed && li > 0 && li + 1 < cnn->layers.size()) {
-                // 2x2 / stride-2 'valid' pooling in front of a convolution the direct kernel takes: the maximum is taken in that
-                // kernel's slab fill (conv_gemm_tc_f16d.cu, IN_POOL) and this layer never runs.  ISS_B200_FUSE_POOL=0: A/B tests.
+                // 2x2 / stride-2 'valid' pooling in front of a convolution the fp16-split engine takes: the maximum is taken in
+                // its operand fill (conv_gemm_tc.cu, LD_POOL) and this layer never runs.  ISS_B200_FUSE_POOL=0: A/B tests.
                 const char *pool_env = getenv("ISS_B200_FUSE_POOL");
                 const bool pool_off = pool_env && pool_env[0] == '0';
                 const Layer &Nx = cnn->layers[li + 1];
@@ -680,7 +676,7 @@ extern "C" int iss_cnn_forward(iss_ctx *ctx, iss_cnn *cnn, const float *d_mspec,
                     pn.in_packed = 1;
                     pn.flags = Nx.d.flags & ~ISS_F_SOFTMAX;
                     pn.pool_h = Lr.in_h; pn.pool_w = Lr.in_w;
-                    if (iss_conv_f16_direct_covers(pn)) { pend_pool_h = Lr.in_h; pend_pool_w = Lr.in_w; continue; }
+                    if (iss_conv_f16_covers(pn)) { pend_pool_h = Lr.in_h; pend_pool_w = Lr.in_w; continue; }
                 }
             }
             if (d.kind == ISS_LAYER_MAXPOOL) {
@@ -713,25 +709,26 @@ extern "C" int iss_cnn_forward(iss_ctx *ctx, iss_cnn *cnn, const float *d_mspec,
                 a.in_packed = cur_packed ? 1 : 0;
                 const bool direct = li == 0 && d.kind == ISS_LAYER_CONV2D && d.cin == 1 &&
                                     (d.cout == 16 || d.cout == 32 || d.cout == 64 || d.cout == 128) && !(d.flags & ISS_F_SOFTMAX);
-                // only the direct first-layer kernel and the fp16-split slab kernel can emit split-half words
+                // only the direct first-layer kernel and the fp16-split engine can emit split-half words
                 const bool can_pack = direct || (li > 0 && iss_get_gemm_mode() == ISS_GEMM_TC_F16 && f16_engine_covers(Lr, a));
                 a.out_packed = (!last && can_pack && wants_packed_output(cnn, li, nb)) ? 1 : 0;
                 ISS_REQUIRE(!a.in_packed || (li > 0 && f16_engine_covers(Lr, a)), ISS_ERR_UNSUPPORTED,
                             "iss_cnn_forward: layer %d was handed split-half words it cannot read", (int)li);
                 int rc;
-                // Fold the first layer into the next convolution's slab fill (FirstFuse, conv_gemm.cuh)?  Needs: the direct
-                // first-layer shape without padding / stride, a packed-input slab convolution right behind it, and a batch
-                // whose patches span few enough frames for the float64 map.
+                // Fold the first layer into the next convolution's operand fill (FirstFuse, conv_gemm.cuh)?  Needs: the direct
+                // first-layer shape without padding / stride, an fp16-split convolution right behind it that takes it, and a
+                // batch whose patches span few enough frames for the float64 map.
                 const char *fuse_env = getenv("ISS_B200_FUSE_FIRST");      // "0" = keep the stand-alone first-layer kernel (A/B tests)
                 const bool fuse_off = fuse_env && fuse_env[0] == '0';
-                bool next_is_direct = false;                     // the FIRST mode lives in the direct kernel only
+                bool next_is_direct = false;                     // the fused first layer lives in the fp16-split engine only
                 if (li == 0 && cnn->layers.size() > 1 && cnn->layers[1].d.kind == ISS_LAYER_CONV2D &&
                     cnn->layers[1].d.pad_bottom == 0 && cnn->layers[1].d.pad_right == 0 && iss_get_gemm_mode() == ISS_GEMM_TC_F16) {
                     ConvArgs p1 = {};
                     fill_conv_args(cnn->layers[1], nb, p1);
                     p1.in_packed = 1;
                     p1.flags = cnn->layers[1].d.flags & ~ISS_F_SOFTMAX;
-                    next_is_direct = iss_conv_f16_direct_covers(p1);
+                    p1.first = &ffuse;
+                    next_is_direct = iss_conv_f16_covers(p1);
                 }
                 if (li == 0 && direct && a.out_packed && !fuse_off && d_first_yh && ranges_ascending && next_is_direct && d.sh == 1 && d.sw == 1 && d.pad_top == 0 && d.pad_left == 0 &&
                     d.pad_bottom == 0 && d.pad_right == 0 && !(d.flags & (ISS_F_SOFTMAX | ISS_F_SIGMOID))) {
@@ -765,7 +762,7 @@ extern "C" int iss_cnn_forward(iss_ctx *ctx, iss_cnn *cnn, const float *d_mspec,
                         f.Hp = Lr.in_h + d.pad_top + d.pad_bottom; f.Wp = Lr.in_w + d.pad_left + d.pad_right;
                         f.Cout = d.cout; f.flags = a.flags; f.out_packed = a.out_packed;
                         const size_t smem = ((size_t)d.kh * d.kw * d.cout + (size_t)f.Hp * f.Wp + FIRST_P * d.sw + d.kw + 8) * sizeof(float);
-                        ISS_REQUIRE(smem <= 200 * 1024, ISS_ERR_UNSUPPORTED, "iss_cnn_forward: first layer too large for the direct kernel");
+                        ISS_REQUIRE(smem <= 200 * 1024, ISS_ERR_UNSUPPORTED, "iss_cnn_forward: first layer too large for the first-layer kernel");
                         ISS_CUDA_OK(iss_optin_smem(reinterpret_cast<const void *>(conv_first_direct_kernel), 200 * 1024));
                         const unsigned grid = (unsigned)std::min<int64_t>(nb, (int64_t)ctx->sm_count * 8);
                         conv_first_direct_kernel<<<grid, 256, smem, st>>>(f);

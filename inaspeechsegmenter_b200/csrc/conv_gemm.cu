@@ -250,7 +250,7 @@ int iss_launch_conv(const ConvArgs &a, bool first, cudaStream_t st)
 {
     if (!first && small_n_covers(a)) {
         const int64_t gm = (a.M + 7) / 8;
-        dense_small_n_kernel<<<(unsigned)(gm < 148 * 8 ? gm : 148 * 8), 256, (size_t)a.K * a.N * sizeof(float), st>>>(a);
+        dense_small_n_kernel<<<(unsigned)(gm < 132 * 8 ? gm : 132 * 8), 256, (size_t)a.K * a.N * sizeof(float), st>>>(a);
         ISS_CUDA_OK(cudaGetLastError());
         iss_count_launch();
         return ISS_OK;

@@ -29,7 +29,7 @@ __device__ __forceinline__ float iss_unpack_split(uint32_t w)
 
 #define ISS_F_RESIDUAL 64     /* internal: + residual[m][n] after the pre-affine, before ReLU */
 
-// First layer folded into the slab fill of the convolution behind it (conv_gemm_tc_f16d.cu, FIRST mode): the
+// First layer folded into the operand fill of the convolution behind it (conv_gemm_tc.cu, LD_FIRST): the
 // first Conv2D of the segmenter CNNs has ONE input channel and its input is the z-normalised patch
 // (x - mu_j) / sigma_j (segmenter.py:82), so by linearity
 //     conv(x^)[t, f, c] = (Y[row0_j + t, f, c] - mu_j * S_c) / sigma_j,   Y = conv(raw log-mel), S_c = sum of the filter
@@ -38,7 +38,7 @@ __device__ __forceinline__ float iss_unpack_split(uint32_t w)
 // (scale s_c, shift t_c) fold with the normalisation into ONE multiply-add per value,
 //     a[t, f, c] = Y * alpha_jc + beta_jc,   alpha_jc = s_c / sigma_j,   beta_jc = (b_c s_c + t_c) - mu_j S_c alpha_jc,
 // with alpha rounded to float32 FIRST and beta (float64, stored as two floats) computed from the rounded alpha, so the
-// cancellation between Y alpha and beta is exact to ~1e-7 relative (first_coef_kernel).  The slab fill evaluates
+// cancellation between Y alpha and beta is exact to ~1e-7 relative (first_coef_kernel).  The operand fill evaluates
 // fma(Yh, alpha, beta_h) + fma(Yl, alpha, beta_l), ReLU, the optional second affine, and writes fp16 hi / lo planes
 // straight into shared memory: the first layer's output (283 KB per patch, 47 % of all activation traffic) never
 // exists in HBM.
@@ -70,23 +70,18 @@ struct ConvArgs {
     const int32_t *row0; const float *mu; const float *sigma;
     // tensor-core path: weights transposed + split, [N][Kp] each (nullptr => fp32 CUDA-core kernel)
     const float *wt_hi; const float *wt_lo; const float *wt_tiled; int Kp;
-    // fp16-split engine (conv_gemm_tc_f16.cu): tiled fp16 hi/lo weight image (nullptr => not prepared) and its scale
+    // fp16-split engine (engine 3, conv_gemm_tc.cu): tiled fp16 hi/lo weight image (nullptr => not prepared) and its scale
     const void *wt_f16; float wt_f16_inv_scale;
     // activation formats of that engine: fp32 values (0) or split-half words lo16 << 16 | hi16 (1)
     int in_packed, out_packed;
     int residual_packed;    // `residual` holds split-half words (fp16-split kernels only)
-    int pool_h, pool_w;     // direct kernel only, > 0: `in` is the un-pooled [n][pool_h][pool_w][C] tensor, 2x2 / stride-2 max taken in the slab fill
-    const FirstFuse *first;         // host pointer, non-null: FIRST mode of the direct kernel (copied into the kernel parameters)
-    // slab kernel (conv_gemm_tc_f16.cu) only, filled in by iss_launch_conv_tc_f16
-    int slab_R;             // output rows (of width OW) per 128-row GEMM tile
-    int slab_rows;          // input rows the slab is sized for
-    int slab_tpi;           // > 0: tiles per image (tiles never straddle images); 0: tiles over the global row sequence
-    int64_t in_elems;       // floats in `in` (loads past the end are zero-filled)
+    int pool_h, pool_w;     // engine 3 only, > 0: `in` is the un-pooled [n][pool_h][pool_w][C] tensor, 2x2 / stride-2 max taken in the operand fill
+    const FirstFuse *first;         // host pointer, non-null: the fused first layer (copied into the kernel parameters)
 };
 
 #define ISS_GEMM_FP32  0      /* fp32 CUDA cores (conv_gemm.cu) */
-#define ISS_GEMM_TC_TS 2      /* tcgen05 3xTF32 (kind::tf32), A from tensor memory, B from shared memory: every layer shape */
-#define ISS_GEMM_TC_F16 3     /* fp16 hi/lo split on kind::f16 for the un-padded stride-1 slab convolutions (conv_gemm_tc_f16.cu); other layers as engine 2 */
+#define ISS_GEMM_TC_TS 2      /* wgmma 3xTF32 (conv_gemm_tc.cu): every layer shape with C, K, N multiples of 32 */
+#define ISS_GEMM_TC_F16 3     /* wgmma fp16 hi/lo split (conv_gemm_tc.cu) for layers with C, N multiples of 64; other layers as engine 2 */
 #ifndef ISS_GEMM_DEFAULT
 #define ISS_GEMM_DEFAULT ISS_GEMM_TC_F16
 #endif
@@ -98,13 +93,8 @@ int iss_launch_conv_tc(const ConvArgs &a, int mode, cudaStream_t st);
 int iss_prepare_tc_weights(const float *h_w, int K, int N, float **d_out, int *Kp_out);
 // W[K][N] -> fp16 hi/lo image of engine 3 (*d_out stays nullptr when the shape is not one that engine takes)
 int iss_prepare_f16_weights(const float *h_w, int K, int N, void **d_out, float *inv_scale);
-// does engine 3's slab kernel cover this layer (geometry + prepared image + shared memory)?
-bool iss_conv_f16_slab_covers(const ConvArgs &a);
-// does engine 3's direct kernel (conv_gemm_tc_f16d.cu: both operands from shared memory) cover this layer?  It reads
-// split-half words (a.in_packed) or, with a.first set, evaluates the one-channel first layer in its slab fill
-bool iss_conv_f16_direct_covers(const ConvArgs &a);
-// does engine 3's gather kernel (conv_gemm_tc_f16g.cu: any stride / padding / 1x1) cover this layer?
-bool iss_conv_f16_gather_covers(const ConvArgs &a);
+// does engine 3 take this layer (weight image, channel counts, the input format / folded pooling / fused first layer)?
+bool iss_conv_f16_covers(const ConvArgs &a);
 // n-tile width of engine 3 for N output channels (must agree between the weight image and the launch)
 int iss_f16_bn_for(int N);
 

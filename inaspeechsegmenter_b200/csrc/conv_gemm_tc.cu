@@ -1,339 +1,350 @@
-// conv_gemm_tc.cu -- implicit-GEMM convolution / dense layer on the 5th-gen tensor
-// cores (tcgen05.mma, accumulators in TMEM) with fp32-class accuracy ("3xTF32"), for every layer
-// shape: padded / strided / 1x1 convolutions (ResNet101) and Dense layers.  The un-padded stride-1
-// KHxKW convolutions of the segmenter CNNs take the faster fp16-split slab kernel of
-// conv_gemm_tc_f16.cu (engine 3, the default) and only fall back to this kernel when it does not
-// cover them.
+// conv_gemm_tc.cu -- implicit-GEMM convolution / dense layer on the Hopper tensor cores (wgmma.mma_async, fp32
+// accumulators in registers) with fp32-class accuracy, for every layer shape the tensor-core engines take: padded /
+// strided / 1x1 convolutions (ResNet101), the KHxKW convolutions of the segmenter CNNs and Dense layers.
 //
-// Why 3xTF32: the reference evaluates its CNNs in fp32 (TF-CPU) and the parity bar is
-// 1e-4 on the per-frame softmax; a single TF32 pass (10-bit mantissa) misses it.  Every
-// fp32 operand x is split exactly into hi = x with the 13 low mantissa bits cleared (a
-// valid TF32 number) and lo = x - hi; the product is accumulated as
+// Every fp32 operand x is split exactly into a high part and a low part and the product is accumulated as
 //      A.B ~= Ah.Bh + Ah.Bl + Al.Bh          (dropped Al.Bl ~ 2^-22 relative)
-// Tile: 128 output positions (UMMA_M = 128, cta_group::1) x BN output channels, K in blocks of 32 floats
-// (= one 128-byte swizzle row); 4 producer/epilogue warps + 1 TMEM-allocator / B-loader / MMA-issuer warp.
-// A operand: cp.async im2col gathers -> warp-private ring -> registers -> hi/lo split -> TMEM (tcgen05.st);
-// weights: one bulk copy per stage of host-pre-swizzled tiles; two accumulators (main + correction).
+// in two accumulators (D_main = Ah.Bh, D_lo = the two correction products) that are added in the epilogue.  Two engines:
+//   engine 2 (3xTF32): hi = x with the 13 low mantissa bits cleared (a valid TF32 number), lo = x - hi; wgmma kind tf32.
+//   engine 3 (fp16 split, the default): hi = fp16(x), lo = fp16(x - hi) (22 significant bits, like the TF32 split) on the
+//       f16 tensor-core path, which runs at twice the TF32 rate.  The weights of a layer are pre-scaled by an exact power of
+//       two so that max|w| lands in [2^12, 2^13) (undone in the epilogue); activations are used as they are, so
+//       |activation| must stay below 65504 (true after BatchNorm / z-normalisation; a network that violates it must use
+//       engine 2).
+// Why the split: the reference evaluates its CNNs in fp32 and the parity bar is 1e-4 on the per-frame softmax; a single
+// TF32 or fp16 pass (10-bit mantissa) misses it.
+//
+// PACKED activations ("split-half words", conv_gemm.cuh): a layer whose consumer is another engine-3 convolution stores
+// every activation as ONE 32-bit word lo16 << 16 | hi16, so that the split is done once per element in the producing
+// epilogue instead of KH*KW times in the consumers' operand fill.  The value carried between layers is hi + lo, exactly
+// what the tensor cores would have used anyway.  Engine 3 also takes a 2x2 / stride-2 max-pooling in front of the
+// convolution (the window maximum is taken in the operand fill, the pooling layer never runs) and the fused first layer of
+// the segmenter CNNs (FirstFuse, conv_gemm.cuh: the first layer's output is evaluated in the operand fill from the
+// float64 map Y and never exists in HBM).
+//
+// Tile: 128 output positions x BN output channels, K in blocks of one 128-byte operand row (32 TF32 / 64 fp16 values).
+// Two warpgroups of 128 threads, each owns 64 GEMM rows: it gathers its rows of the k-block (im2col, one 16-byte chunk of
+// the operand row per thread and row), splits them and writes hi / lo into a double-buffered SWIZZLE_128B tile, then
+// issues its wgmmas.  The weights are static, so the host stores them already tiled and swizzled exactly as the shared
+// memory operand image ([n-tile][k-block][hi|lo][BN rows x 128 B]); all 256 threads copy a stage with cp.async, four
+// stages deep (two k-blocks ahead).  The global loads of k-block kb+1 are in flight while the wgmmas of kb are issued,
+// and wgmma.wait_group 1 keeps one k-block of tensor work running while the next tile is filled.
 #include <cuda.h>
+#include <cuda_fp16.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
+
 #include <vector>
 
 #include "conv_gemm.cuh"
-
+#include "f16_image.cuh"
 #include "tc_common.cuh"
 
 namespace {
 
-// ---------------------------------------------------------------------------------------------
-// B loader + MMA issuer, run by ALL 32 lanes of warp 4 with warp-uniform control flow; only the
-// tcgen05 / bulk-copy instructions themselves sit under elect.sync.  This matters more than anything
-// else in the kernel: with the loop inside `if (lane == 0)` ptxas cannot prove the tcgen05 operands
-// (TMEM addresses, smem descriptors) warp-uniform and wraps EVERY tcgen05.mma in an
-// ELECT / 4 x R2UR.BROADCAST / BRA.U.ANY "waterfall" -- ~50 issue cycles per MMA, ~330 instructions per
-// k-block on one thread, i.e. 600-1100 cycles per k-block against a tensor-time floor of 392 (measured with
-// what-if builds in round 1, profiles/r01_tc_whatif.txt).  With uniform control flow and the TMEM base
-// passed through REDUX (a uniform-register producer) the 8 MMAs of a k-block are 8 back-to-back UTCHMMA.
-// The weights are static, so the host stores them already tiled and swizzled exactly as the smem operand
-// image ([n-tile][k-block][hi|lo][BN x 128 B, SWIZZLE_128B]); one stage is a single 1-D bulk copy.
-template <int BN, int SB, int ST, int B_STAGE, uint32_t ACC_COLS>
-__device__ __forceinline__ void tc_issuer_warp(const ConvArgs &a, uint32_t tmem_base_any, unsigned char *b_ring, uint64_t *fullA,
-                                               uint64_t *emptyA, uint64_t *fullB, uint64_t *emptyB, uint64_t *accum, int nkb)
-{
-    constexpr uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(TBM >> 4) << 24);
-    constexpr uint32_t idesc2 = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)((2 * BN) >> 3) << 17) | ((uint32_t)(TBM >> 4) << 24);
-    const uint32_t tmem_base = __reduce_or_sync(0xffffffffu, tmem_base_any);
-    const unsigned char *wt = reinterpret_cast<const unsigned char *>(a.wt_tiled) + (size_t)blockIdx.y * nkb * B_STAGE;
-    auto issue_b = [&](int kb) {
-        if (kb < nkb) {
-            const int sl = kb % SB;
-            if (elect_one()) {
-                asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(&fullB[sl])), "r"((uint32_t)B_STAGE) : "memory");
-                asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                             ::"r"(smem_u32(b_ring + sl * B_STAGE)), "l"(wt + (size_t)kb * B_STAGE),
-                               "r"((uint32_t)B_STAGE), "r"(smem_u32(&fullB[sl])) : "memory");
-            }
-            __syncwarp();
-        }
-    };
-    for (int p = 0; p < SB - 1; ++p) issue_b(p);
-    const uint32_t d_main = tmem_base, d_lo = tmem_base + BN;
-    for (int kb = 0; kb < nkb; ++kb) {
-        const int st = kb % ST, sl = kb % SB;
-        mbar_wait(&fullB[sl], (kb / SB) & 1, 2);
-        mbar_wait(&fullA[st], (kb / ST) & 1, 3);
-        tc_fence_after();
-        const uint64_t dbh = make_sw128_desc(smem_u32(b_ring + sl * B_STAGE));
-        const uint32_t ta = tmem_base + ACC_COLS + st * 2 * TBK;
-        if (elect_one()) {
-            // the B stage is [hi rows | lo rows] and the accumulators are [D_main | D_lo] in adjacent TMEM
-            // columns, hence Ah.Bh and Ah.Bl are ONE MMA of width 2*BN (D_main += Ah.Bh, D_lo += Ah.Bl);
-            // Al.Bh follows into D_lo.
-#pragma unroll
-            for (int kk = 0; kk < TBK / 8; ++kk) {
-                const uint32_t first = (kb > 0 || kk > 0) ? 1u : 0u;
-                umma_tf32_ts(d_main, ta + kk * 8, dbh + 2 * kk, idesc2, first);          // Ah.[Bh | Bl]
-                umma_tf32_ts(d_lo, ta + TBK + kk * 8, dbh + 2 * kk, idesc, 1u);          // Al.Bh
-            }
-            umma_commit(&emptyA[st]);
-            umma_commit(&emptyB[sl]);
-            if (kb == nkb - 1) umma_commit(accum);
-        }
-        __syncwarp();
-        // refill the slot of k-block kb-1 with kb+SB-1: its MMAs retire before those just issued start,
-        // so this wait is short and the tensor pipe is never drained
-        if (kb + SB - 1 < nkb) {
-            if (kb >= 1) mbar_wait(&emptyB[(kb - 1) % SB], ((kb - 1) / SB) & 1, 4);   // slot (kb-1)%SB; unused so far when kb == 0
-            issue_b(kb + SB - 1);
-        }
-    }
-}
+constexpr int TBM = 128, TBK = 32, HBK = 64;
+constexpr int THREADS = 256;
+constexpr int A_WG = 16384;                  // one warpgroup's operand tile of one stage: hi | lo, 64 rows x 128 B each
+constexpr int A_STAGES = 2, B_STAGES = 4;
 
-// ---------------------------------------------------------------------------------------------
-// Asynchronous TS pipeline (the production path).  Differences from the kernel above:
-//   * A rows are fetched with cp.async (16-byte, L2 -> smem, zero-fill for padding / tail rows)
-//     into a warp-private DA-deep ring, so DA k-blocks of gathers are in flight per warp with no
-//     register staging; the ring doubles as the transpose buffer (lane = row on the way out).
-//   * the weight tiles are fetched by the MMA warp itself (32 lanes of cp.async into an SB-deep
-//     ring), which removes them from the producers' critical path;
-//   * operand A goes registers -> TMEM (tcgen05.st) into an ST-deep ring next to the two
-//     accumulators, so shared memory only carries B for the MMAs.
-template <int BN, int DA, int SB, int ST>
-struct Tc2Cfg {
-    static constexpr int A_SLOT = 4096;                                  // 32 rows x 128 B per warp
-    static constexpr int A_RING = 4 * DA * A_SLOT;
-    static constexpr int THREADS = 160;
-    static constexpr int B_TILE = BN * TBK * 4;
-    static constexpr int B_STAGE = 2 * B_TILE;                           // hi | lo
-    static constexpr int SMEM = A_RING + SB * B_STAGE + 1024 + 256;
-    static constexpr uint32_t ACC_COLS = 2 * BN;
-    static constexpr uint32_t TMEM_COLS = tmem_cols_pow2(ACC_COLS + ST * 2 * TBK);
+constexpr int ENG_TF32 = 0, ENG_F16 = 1;
+// operand fill of engine 3: fp32 values split here, split-half words, words with the 2x2 max-pooling in front, or the
+// fused first layer.  Engine 2 reads fp32 values only.
+constexpr int LD_F32 = 0, LD_PACKED = 1, LD_POOL = 2, LD_FIRST = 3;
+
+template <int BN>
+struct WgCfg {
+    static constexpr int B_STAGE = 2 * BN * 128;                         // hi | lo, BN rows x 128 B each
+    static constexpr int SMEM = B_STAGES * B_STAGE + A_STAGES * 2 * A_WG + 1024;
 };
 
-template <int BN, int DA, int SB, int ST>
-__global__ void __launch_bounds__(160, (Tc2Cfg<BN, DA, SB, ST>::TMEM_COLS <= 256 ? 2 : 1))
-conv_gemm_tc2_kernel(const ConvArgs a)
+__device__ __forceinline__ void split_f16(const float (&v)[8], uint32_t (&hw)[4], uint32_t (&lw)[4])
 {
-    using Cfg = Tc2Cfg<BN, DA, SB, ST>;
-    extern __shared__ unsigned char smem_dyn[];
-    unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
-    unsigned char *b_ring = smem;                                        // 1024-aligned operand tiles first
-    unsigned char *a_ring = smem + SB * Cfg::B_STAGE;
-    uint64_t *bars = reinterpret_cast<uint64_t *>(a_ring + Cfg::A_RING);
-    uint64_t *fullA = bars, *emptyA = bars + ST, *emptyB = bars + 2 * ST, *fullB = bars + 2 * ST + SB, *accum = bars + 2 * ST + 2 * SB;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bars + 2 * ST + 2 * SB + 1);
-
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int64_t m0 = (int64_t)blockIdx.x * TBM;
-    const int n0 = blockIdx.y * BN;
-    const int nkb = a.Kp / TBK;
-
-    if (tid == 0) {
-        for (int s = 0; s < ST; ++s) { mbar_init(&fullA[s], 4); mbar_init(&emptyA[s], 1); }
-        for (int s = 0; s < SB; ++s) { mbar_init(&emptyB[s], 1); mbar_init(&fullB[s], 1); }
-        mbar_init(accum, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 4) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(Cfg::TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp != 4) {
-        // ============================ A producers ============================
-        const int quad = warp & 3;                           // TMEM lane quadrant this warp may access
-        // Issue-slot budget matters here (the kernel is instruction-issue bound before it is tensor
-        // bound): per-row state is 32-bit and precomputed, the filter tap advances incrementally
-        // (no integer division in the loop) and un-padded convolutions skip all bounds checks.
-        const int sub = lane >> 3, chunk = lane & 7;
-        uint32_t row_base[8];                                // element offset of (img, ih0, iw0) + chunk*4 (wraps for padded rows)
-        int row_ih0[8], row_iw0[8];
-        uint32_t row_dst[8];                                 // swizzled byte offset inside a ring slot
-        uint32_t ok_mask = 0;
 #pragma unroll
-        for (int i = 0; i < 8; ++i) {
-            const int64_t m = m0 + quad * 32 + 4 * i + sub;
-            const bool okr = m < a.M;
-            ok_mask |= (okr ? 1u : 0u) << i;
-            const int64_t mm = okr ? m : 0;
-            const int ohw = a.OH * a.OW;
-            const int64_t img = mm / ohw;
-            const int rem = (int)(mm - img * ohw);
-            const int oh = rem / a.OW, ow = rem - oh * a.OW;
-            row_ih0[i] = oh * a.SH - a.PT; row_iw0[i] = ow * a.SW - a.PL;
-            row_base[i] = (uint32_t)(img * ((int64_t)a.H * a.W * a.C) + ((int64_t)row_ih0[i] * a.W + row_iw0[i]) * a.C + chunk * 4);
-            const int rl = 4 * i + sub;
-            row_dst[i] = (uint32_t)(rl * 128 + ((chunk ^ (rl & 7)) << 4));
-        }
-        const bool padded = (a.PT | a.PL) != 0 || (a.OH - 1) * a.SH + a.KH > a.H || (a.OW - 1) * a.SW + a.KW > a.W;
-        unsigned char *my_ring = a_ring + quad * DA * Cfg::A_SLOT;
-        const uint32_t ring_u32 = smem_u32(my_ring);
-        // incremental tap state of the next k-block to gather
-        int is_c0 = 0, is_ss = 0, is_rr = 0, is_kb = 0, is_n = 0;
-        uint32_t is_off = 0;                                 // (rr*W + ss)*C + c0
-        const uint32_t wrap_step = (uint32_t)((a.W - a.KW) * a.C + TBK);
-        auto advance = [&]() {
-            ++is_kb;
-            is_c0 += TBK; is_off += TBK;
-            if (is_c0 == a.C) {
-                is_c0 = 0;
-                if (++is_ss == a.KW) { is_ss = 0; ++is_rr; is_off += wrap_step - TBK; }
-            }
-        };
-        auto issue_a = [&]() {
-            if (is_kb < nkb) {
-                const uint32_t slot = ring_u32 + (uint32_t)(is_n % DA) * Cfg::A_SLOT;
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                    bool ok = (ok_mask >> i) & 1u;
-                    if (padded) {
-                        const int ih = row_ih0[i] + is_rr, iw = row_iw0[i] + is_ss;
-                        ok = ok && ih >= 0 && ih < a.H && iw >= 0 && iw < a.W;
-                    }
-                    const float *src = a.in + (ok ? (uint32_t)(row_base[i] + is_off) : 0u);
-                    // .cg (L2 only); L1-allocating gathers (.ca) measured no different
-                    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(slot + row_dst[i]), "l"(src), "r"(ok ? 16 : 0) : "memory");
-                }
-                ++is_n;
-                advance();
-            }
-            cp_async_commit();
-        };
-#pragma unroll
-        for (int p = 0; p < DA; ++p) issue_a();
-        const uint32_t lane_addr = ((uint32_t)(quad * 32)) << 16;
-        uint32_t lds_off[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) lds_off[j] = (uint32_t)(lane * 128 + ((j ^ (lane & 7)) << 4));
-        // Software pipeline: the TMEM stores of k-block kb are issued, then the ring slot of kb+1 is
-        // read and split while they drain; only then tcgen05.wait::st + arrive.  The per-warp critical
-        // path per k-block is max(store latency, load+split) instead of their sum.
-        uint32_t hi[32], lo[32];
-        auto load_split = [&](int n) {                        // n-th k-block of this set
-            cp_async_wait<DA - 1>();
-            __syncwarp();
-            const unsigned char *slot = my_ring + (n % DA) * Cfg::A_SLOT;
-            uint32_t v[32];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                const uint4 q = *reinterpret_cast<const uint4 *>(slot + lds_off[j]);
-                v[4 * j] = q.x; v[4 * j + 1] = q.y; v[4 * j + 2] = q.z; v[4 * j + 3] = q.w;
-            }
-            __syncwarp();                                    // slot fully read before it is refilled
-            issue_a();
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-                hi[j] = v[j] & 0xFFFFE000u;
-                lo[j] = __float_as_uint(__uint_as_float(v[j]) - __uint_as_float(hi[j]));
-            }
-        };
-        load_split(0);
-        int nloc = 0;
-        for (int kb = 0; kb < nkb; ++kb, ++nloc) {
-            const int st = kb % ST;
-            if (lane == 0) mbar_wait(&emptyA[st], ((kb / ST) & 1) ^ 1, 1);   // one poller / one arrival per warp:
-            __syncwarp();                                                     // 128 threads hammering the mbarriers cost more than the MMAs
-            tc_fence_after();
-            const uint32_t ta = tmem_base + lane_addr + Cfg::ACC_COLS + st * 2 * TBK;
-            tmem_st32(ta, hi);
-            tmem_st32(ta + TBK, lo);
-            if (kb + 1 < nkb) load_split(nloc + 1);       // overlaps the TMEM store latency
-            asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&fullA[st]);
-        }
-        cp_async_wait<0>();
-
-        // ============================ epilogue ============================
-        if (lane == 0) mbar_wait(accum, 0, 5);
-        __syncwarp();
-        tc_fence_after();
-        unsigned char *stage_buf = my_ring;                  // the A ring is idle now: reuse slot 0 as transpose buffer
-        const bool has_bias = a.flags & ISS_F_BIAS, pre = a.flags & ISS_F_AFFINE_PRE, post = a.flags & ISS_F_AFFINE_POST;
-        const bool relu = a.flags & ISS_F_RELU, resid = a.flags & ISS_F_RESIDUAL;
-#pragma unroll 1
-        for (int c = 0; c < BN; c += 32) {
-            uint32_t acc[32];
-            {
-                uint32_t corr[32];
-                tmem_ld32(tmem_base + lane_addr + c, acc);
-                tmem_ld32(tmem_base + lane_addr + BN + c, corr);
-#pragma unroll
-                for (int j = 0; j < 32; ++j) acc[j] = __float_as_uint(__uint_as_float(acc[j]) + __uint_as_float(corr[j]));
-            }
-            __syncwarp();
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-                *reinterpret_cast<uint4 *>(stage_buf + lane * 128 + ((j ^ (lane & 7)) << 4)) =
-                    make_uint4(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]);
-            __syncwarp();
-            const int nb = n0 + c + chunk * 4;
-            float eb[4], es1[4], et1[4], es2[4], et2[4];
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-                eb[q] = has_bias ? __ldg(a.bias + nb + q) : 0.f;
-                es1[q] = pre ? __ldg(a.pre_scale + nb + q) : 1.f;  et1[q] = pre ? __ldg(a.pre_shift + nb + q) : 0.f;
-                es2[q] = post ? __ldg(a.post_scale + nb + q) : 1.f; et2[q] = post ? __ldg(a.post_shift + nb + q) : 0.f;
-            }
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                const int rl = 4 * i + sub;
-                const int64_t m = m0 + quad * 32 + rl;
-                const uint4 q4 = *reinterpret_cast<const uint4 *>(stage_buf + rl * 128 + ((chunk ^ (rl & 7)) << 4));
-                if (m < a.M) {
-                    float y[4] = {__uint_as_float(q4.x), __uint_as_float(q4.y), __uint_as_float(q4.z), __uint_as_float(q4.w)};
-                    float4 rs = make_float4(0.f, 0.f, 0.f, 0.f);
-                    if (resid) rs = __ldg(reinterpret_cast<const float4 *>(a.residual + m * a.N + nb));
-                    const float rv[4] = {rs.x, rs.y, rs.z, rs.w};
-#pragma unroll
-                    for (int q = 0; q < 4; ++q) {
-                        float t = y[q] + eb[q];
-                        if (pre) t = fmaf(t, es1[q], et1[q]);
-                        if (resid) t += rv[q];
-                        if (relu) t = fmaxf(t, 0.f);
-                        if (post) t = fmaf(t, es2[q], et2[q]);
-                        y[q] = t;
-                    }
-                    *reinterpret_cast<float4 *>(a.out + m * a.N + nb) = make_float4(y[0], y[1], y[2], y[3]);
-                }
-            }
-        }
-        tc_fence_before();
-    } else {
-        // ============================ B loader + MMA issuer (warp 4) ============================
-        tc_issuer_warp<BN, SB, ST, Cfg::B_STAGE, Cfg::ACC_COLS>(a, tmem_base, b_ring, fullA, emptyA, fullB, emptyB, accum, nkb);
-        tc_fence_before();
-    }
-    __syncthreads();
-    if (warp == 4) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(Cfg::TMEM_COLS) : "memory");
+    for (int e = 0; e < 4; ++e) {                            // hi = fp16(v), lo = fp16(v - hi): even k in the low half
+        const __half2 hh = __floats2half2_rn(v[2 * e], v[2 * e + 1]);
+        const float2 hf = __half22float2(hh);
+        const __half2 ll = __floats2half2_rn(v[2 * e] - hf.x, v[2 * e + 1] - hf.y);
+        hw[e] = *reinterpret_cast<const uint32_t *>(&hh);
+        lw[e] = *reinterpret_cast<const uint32_t *>(&ll);
     }
 }
 
-
-constexpr int SMEM_CTA_MAX = 232448;       // 227 KB opt-in limit per CTA
-constexpr int SMEM_HALF_SM = 115712;       // two CTAs per SM: 2 * (x + 1 KB reserved) <= 228 KB
-
-template <int BN, int DA, int SB, int ST>
-int launch_tc2(const ConvArgs &a, cudaStream_t st)
+__device__ __forceinline__ void words_to_planes(const uint32_t (&w)[8], uint32_t (&hw)[4], uint32_t (&lw)[4])
 {
-    using Cfg = Tc2Cfg<BN, DA, SB, ST>;
-    auto kern = conv_gemm_tc2_kernel<BN, DA, SB, ST>;
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {                            // word = lo << 16 | hi; operand column = k even (low) | k odd (high)
+        hw[e] = __byte_perm(w[2 * e], w[2 * e + 1], 0x5410);
+        lw[e] = __byte_perm(w[2 * e], w[2 * e + 1], 0x7632);
+    }
+}
+
+template <int ENG, int BN, int MODE>
+__global__ void __launch_bounds__(THREADS, 1)
+conv_gemm_wg_kernel(const ConvArgs a, const FirstFuse ff, const unsigned char *__restrict__ wt, float inv_scale)
+{
+    using Cfg = WgCfg<BN>;
+    constexpr int KE = ENG == ENG_F16 ? HBK : TBK;                       // k-elements per block
+    constexpr int RAW = ENG == ENG_F16 ? 2 : 1;                          // 16-byte input loads per 16-byte operand chunk
+    constexpr bool PREFETCH = MODE == LD_F32 || MODE == LD_PACKED;       // raw input held in registers one k-block ahead
+    extern __shared__ unsigned char smem_dyn[];
+    unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
+    unsigned char *b_ring = smem;
+    const uint32_t b_ring_u32 = smem_u32(b_ring);
+    const uint32_t a_ring_u32 = b_ring_u32 + B_STAGES * Cfg::B_STAGE;
+
+    const int tid = threadIdx.x, wg = tid >> 7, t = tid & 127;
+    const int64_t m0 = (int64_t)blockIdx.x * TBM + wg * 64;
+    const int n0 = blockIdx.y * BN;
+    const int nkb = a.K / KE;
+    const unsigned char *wtile = wt + (size_t)blockIdx.y * nkb * Cfg::B_STAGE;
+
+    auto issue_b = [&](int kb) {
+        if (kb < nkb) {
+            const unsigned char *src = wtile + (size_t)kb * Cfg::B_STAGE;
+            const uint32_t dst = b_ring_u32 + (uint32_t)(kb % B_STAGES) * Cfg::B_STAGE;
+#pragma unroll
+            for (int o = tid * 16; o < Cfg::B_STAGE; o += THREADS * 16) cp_async16_u32(dst + o, src + o, 16);
+        }
+        cp_async_commit();                                   // (empty groups keep the group count uniform)
+    };
+    issue_b(0);
+    issue_b(1);
+
+    // this thread's operand rows (64 per warpgroup): r_i = t / 8 + 16 i, 16-byte chunk j of the 128-byte operand row
+    const int j = t & 7;
+    int row_img[4], row_ih0[4], row_iw0[4];
+    uint32_t ok_mask = 0;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const int64_t m = m0 + (t >> 3) + 16 * i;
+        const bool okr = m < a.M;
+        ok_mask |= (okr ? 1u : 0u) << i;
+        const int64_t mm = okr ? m : 0;
+        const int64_t ohw = (int64_t)a.OH * a.OW;
+        const int64_t img = mm / ohw;
+        const int rem = (int)(mm - img * ohw);
+        const int oh = rem / a.OW, ow = rem - oh * a.OW;
+        row_img[i] = (int)img;
+        row_ih0[i] = oh * a.SH - a.PT;
+        row_iw0[i] = ow * a.SW - a.PL;
+    }
+    const uint32_t row_dst0 = (uint32_t)((t >> 3) * 128 + ((j ^ ((t >> 3) & 7)) << 4));   // (t/8 + 16 i) & 7 == (t/8) & 7
+    // tap of the next k-block to fill: k = (rr * KW + ss) * C + c0
+    int tap_c0 = 0, tap_ss = 0, tap_rr = 0;
+    auto advance = [&]() {
+        tap_c0 += KE;
+        if (tap_c0 == a.C) { tap_c0 = 0; if (++tap_ss == a.KW) { tap_ss = 0; ++tap_rr; } }
+    };
+    auto pixel_ok = [&](int i, int &ih, int &iw) {
+        ih = row_ih0[i] + tap_rr; iw = row_iw0[i] + tap_ss;
+        return ((ok_mask >> i) & 1u) && ih >= 0 && ih < a.H && iw >= 0 && iw < a.W;
+    };
+
+    uint4 raw[4][RAW];
+    auto fetch = [&]() {                                     // PREFETCH modes: the raw 16-byte chunks of the next k-block
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            int ih, iw;
+            if (pixel_ok(i, ih, iw)) {
+                const uint4 *p = reinterpret_cast<const uint4 *>(
+                    a.in + (((int64_t)row_img[i] * a.H + ih) * a.W + iw) * a.C + tap_c0 + j * (4 * RAW));
+#pragma unroll
+                for (int q = 0; q < RAW; ++q) raw[i][q] = __ldg(p + q);
+            } else {
+#pragma unroll
+                for (int q = 0; q < RAW; ++q) raw[i][q] = make_uint4(0u, 0u, 0u, 0u);
+            }
+        }
+        advance();
+    };
+
+    // split the k-block into the hi / lo tiles of stage s of this warpgroup
+    auto fill = [&](int s) {
+        const uint32_t hi_base = a_ring_u32 + (uint32_t)(s * 2 + wg) * A_WG, lo_base = hi_base + A_WG / 2;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const uint32_t dst = row_dst0 + i * 16 * 128;
+            uint32_t hw[4], lw[4];
+            if constexpr (ENG == ENG_TF32) {
+                const uint32_t v[4] = {raw[i][0].x, raw[i][0].y, raw[i][0].z, raw[i][0].w};
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    hw[e] = v[e] & 0xFFFFE000u;
+                    lw[e] = __float_as_uint(__uint_as_float(v[e]) - __uint_as_float(hw[e]));
+                }
+            } else if constexpr (MODE == LD_F32) {
+                const float v[8] = {__uint_as_float(raw[i][0].x), __uint_as_float(raw[i][0].y), __uint_as_float(raw[i][0].z), __uint_as_float(raw[i][0].w),
+                                    __uint_as_float(raw[i][1].x), __uint_as_float(raw[i][1].y), __uint_as_float(raw[i][1].z), __uint_as_float(raw[i][1].w)};
+                split_f16(v, hw, lw);
+            } else if constexpr (MODE == LD_PACKED) {
+                const uint32_t w[8] = {raw[i][0].x, raw[i][0].y, raw[i][0].z, raw[i][0].w, raw[i][1].x, raw[i][1].y, raw[i][1].z, raw[i][1].w};
+                words_to_planes(w, hw, lw);
+            } else if constexpr (MODE == LD_POOL) {
+                // the 2x2 window of the un-pooled NHWC tensor [img][pool_h][pool_w][C]: the WORD of the largest value is kept
+                // (as maxpool_nhwc_packed_kernel does: window order (0,0) (0,1) (1,0) (1,1), NaN wins, first maximum wins)
+                uint32_t bw[8] = {0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
+                int ih, iw;
+                if (pixel_ok(i, ih, iw)) {
+                    const uint32_t *in = reinterpret_cast<const uint32_t *>(a.in);
+                    const int64_t p00 = (((int64_t)row_img[i] * a.pool_h + 2 * ih) * a.pool_w + 2 * iw) * a.C + tap_c0 + j * 8;
+                    const int64_t offs[4] = {p00, p00 + a.C, p00 + (int64_t)a.pool_w * a.C, p00 + (int64_t)a.pool_w * a.C + a.C};
+                    float bv[8];
+#pragma unroll
+                    for (int q = 0; q < 4; ++q) {
+                        const uint4 u0 = __ldg(reinterpret_cast<const uint4 *>(in + offs[q]));
+                        const uint4 u1 = __ldg(reinterpret_cast<const uint4 *>(in + offs[q]) + 1);
+                        const uint32_t w[8] = {u0.x, u0.y, u0.z, u0.w, u1.x, u1.y, u1.z, u1.w};
+#pragma unroll
+                        for (int e = 0; e < 8; ++e) {
+                            const float fv = iss_unpack_split(w[e]);
+                            if (q == 0 || fv > bv[e] || fv != fv) { bv[e] = fv; bw[e] = w[e]; }
+                        }
+                    }
+                }
+                words_to_planes(bw, hw, lw);
+            } else {                                          // LD_FIRST (C = 64, stride 1, no padding)
+                float v[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+                int ih, iw;
+                if (pixel_ok(i, ih, iw)) {
+                    const int img = row_img[i];
+                    const int64_t o = (((int64_t)__ldg(ff.row0 + img) - ff.y_f0 + ih) * a.W + iw) * HBK + j * 8;
+                    const float4 *yh = reinterpret_cast<const float4 *>(ff.Yh + o), *yl = reinterpret_cast<const float4 *>(ff.Yl + o);
+                    const float4 *cf = reinterpret_cast<const float4 *>(ff.coef + (int64_t)img * (3 * HBK) + j * 8);
+#pragma unroll
+                    for (int q = 0; q < 2; ++q) {
+                        const float4 h4 = __ldg(yh + q), l4 = __ldg(yl + q);
+                        const float4 va = __ldg(cf + q), vh = __ldg(cf + HBK / 4 + q), vl = __ldg(cf + 2 * (HBK / 4) + q);
+                        const float hv[4] = {h4.x, h4.y, h4.z, h4.w}, lv[4] = {l4.x, l4.y, l4.z, l4.w};
+                        const float al[4] = {va.x, va.y, va.z, va.w}, bh[4] = {vh.x, vh.y, vh.z, vh.w}, bl[4] = {vl.x, vl.y, vl.z, vl.w};
+#pragma unroll
+                        for (int e = 0; e < 4; ++e) {
+                            float u = fmaf(hv[e], al[e], bh[e]) + fmaf(lv[e], al[e], bl[e]);
+                            if (ff.flags & ISS_F_RELU) u = fmaxf(u, 0.f);
+                            if (ff.flags & ISS_F_AFFINE_POST) {
+                                const int c = j * 8 + 4 * q + e;
+                                u = fmaf(u, __ldg(ff.post_scale + c), __ldg(ff.post_shift + c));
+                            }
+                            v[4 * q + e] = u;
+                        }
+                    }
+                }
+                split_f16(v, hw, lw);
+            }
+            sts128(hi_base + dst, hw[0], hw[1], hw[2], hw[3]);
+            sts128(lo_base + dst, lw[0], lw[1], lw[2], lw[3]);
+        }
+        if constexpr (!PREFETCH) advance();
+    };
+
+    float dm[BN / 2], dl[BN / 2];
+#pragma unroll
+    for (int q = 0; q < BN / 2; ++q) { dm[q] = 0.f; dl[q] = 0.f; }
+
+    if constexpr (PREFETCH) fetch();
+    for (int kb = 0; kb < nkb; ++kb) {
+        const int s = kb & 1;
+        fill(s);                                             // stage s was last read by this warpgroup's wgmmas of kb - 2
+        if constexpr (PREFETCH) { if (kb + 1 < nkb) fetch(); }
+        cp_async_wait<1>();                                  // weights of kb landed (kb + 1 may still be in flight)
+        fence_proxy_async();
+        __syncthreads();
+        issue_b(kb + 2);                                     // its stage was read by kb - 2, retired in every warpgroup
+        wgmma_fence();
+        const uint64_t da = make_sw128_desc(a_ring_u32 + (uint32_t)(s * 2 + wg) * A_WG);
+        const uint64_t dal = da + ((A_WG / 2) >> 4);
+        const uint64_t db = make_sw128_desc(b_ring_u32 + (uint32_t)(kb % B_STAGES) * Cfg::B_STAGE);
+        const uint64_t dbl = db + ((BN * 128) >> 4);
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {                     // 32 bytes of the operand row per wgmma (k16 fp16 / k8 tf32)
+            if constexpr (ENG == ENG_F16) {
+                wgmma_f16<BN>(dm, da + 2 * kk, db + 2 * kk);     // Ah.Bh
+                wgmma_f16<BN>(dl, da + 2 * kk, dbl + 2 * kk);    // Ah.Bl
+                wgmma_f16<BN>(dl, dal + 2 * kk, db + 2 * kk);    // Al.Bh
+            } else {
+                wgmma_tf32<BN>(dm, da + 2 * kk, db + 2 * kk);
+                wgmma_tf32<BN>(dl, da + 2 * kk, dbl + 2 * kk);
+                wgmma_tf32<BN>(dl, dal + 2 * kk, db + 2 * kk);
+            }
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+    }
+    wgmma_wait<0>();
+    cp_async_wait<0>();
+
+    // ============================ epilogue (from the accumulator registers) ============================
+    const int w = t >> 5, l = t & 31;
+    const int64_t mr = m0 + 16 * w + (l >> 2);
+    const bool has_bias = a.flags & ISS_F_BIAS, pre = a.flags & ISS_F_AFFINE_PRE, post = a.flags & ISS_F_AFFINE_POST;
+    const bool relu = a.flags & ISS_F_RELU, resid = a.flags & ISS_F_RESIDUAL;
+#pragma unroll
+    for (int i = 0; i < BN / 8; ++i) {
+        const int nb = n0 + 8 * i + 2 * (l & 3);
+        float eb[2], es1[2], et1[2], es2[2], et2[2];
+#pragma unroll
+        for (int q = 0; q < 2; ++q) {
+            eb[q] = has_bias ? __ldg(a.bias + nb + q) : 0.f;
+            es1[q] = pre ? __ldg(a.pre_scale + nb + q) : 1.f;  et1[q] = pre ? __ldg(a.pre_shift + nb + q) : 0.f;
+            es2[q] = post ? __ldg(a.post_scale + nb + q) : 1.f; et2[q] = post ? __ldg(a.post_shift + nb + q) : 0.f;
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int64_t m = mr + 8 * h;
+            if (m >= a.M) continue;
+            float y[2] = {dm[4 * i + 2 * h] + dl[4 * i + 2 * h], dm[4 * i + 2 * h + 1] + dl[4 * i + 2 * h + 1]};
+            float rv[2] = {0.f, 0.f};
+            if (resid) {
+                const uint2 rw = __ldg(reinterpret_cast<const uint2 *>(a.residual + m * a.N + nb));
+                if (a.residual_packed) { rv[0] = iss_unpack_split(rw.x); rv[1] = iss_unpack_split(rw.y); }
+                else { rv[0] = __uint_as_float(rw.x); rv[1] = __uint_as_float(rw.y); }
+            }
+#pragma unroll
+            for (int q = 0; q < 2; ++q) {
+                float v;
+                if constexpr (ENG == ENG_F16)                 // ((acc * inv_s) + bias) * s1 + t1 as one multiply-add
+                    v = fmaf(y[q], inv_scale * es1[q], fmaf(eb[q], es1[q], et1[q]));
+                else {
+                    v = y[q] + eb[q];
+                    if (pre) v = fmaf(v, es1[q], et1[q]);
+                }
+                if (resid) v += rv[q];
+                if (relu) v = fmaxf(v, 0.f);
+                if (post) v = fmaf(v, es2[q], et2[q]);
+                y[q] = v;
+            }
+            float *dst = a.out + m * a.N + nb;
+            if (a.out_packed) *reinterpret_cast<uint2 *>(dst) = make_uint2(iss_pack_split(y[0]), iss_pack_split(y[1]));
+            else *reinterpret_cast<float2 *>(dst) = make_float2(y[0], y[1]);
+        }
+    }
+}
+
+template <int ENG, int BN, int MODE>
+int launch_wg(const ConvArgs &a, const void *wt, float inv_scale, cudaStream_t st)
+{
+    using Cfg = WgCfg<BN>;
+    auto kern = conv_gemm_wg_kernel<ENG, BN, MODE>;
     ISS_CUDA_OK(iss_optin_smem(reinterpret_cast<const void *>(kern), Cfg::SMEM));
     const int64_t gm = (a.M + TBM - 1) / TBM;
     ISS_REQUIRE(gm < (1ll << 31), ISS_ERR_INVALID, "conv_tc: M too large");
+    const FirstFuse ff = a.first ? *a.first : FirstFuse{};
     dim3 grid((unsigned)gm, (unsigned)(a.N / BN));
-    kern<<<grid, Cfg::THREADS, Cfg::SMEM, st>>>(a);
+    kern<<<grid, THREADS, Cfg::SMEM, st>>>(a, ff, reinterpret_cast<const unsigned char *>(wt), inv_scale);
     ISS_CUDA_OK(cudaGetLastError());
     iss_count_launch();
     return ISS_OK;
+}
+
+template <int BN>
+int launch_f16(const ConvArgs &a, cudaStream_t st)
+{
+    const float s = a.wt_f16_inv_scale;
+    if (a.first) return launch_wg<ENG_F16, BN, LD_FIRST>(a, a.wt_f16, s, st);
+    if (a.pool_h > 0) return launch_wg<ENG_F16, BN, LD_POOL>(a, a.wt_f16, s, st);
+    if (a.in_packed) return launch_wg<ENG_F16, BN, LD_PACKED>(a, a.wt_f16, s, st);
+    return launch_wg<ENG_F16, BN, LD_F32>(a, a.wt_f16, s, st);
 }
 
 int g_gemm_mode = -1;      // -1 = read ISS_B200_GEMM on first use
@@ -359,44 +370,44 @@ extern "C" int iss_get_gemm_mode(void)
     return g_gemm_mode;
 }
 
-int iss_launch_conv_tc_f16(ConvArgs &a, cudaStream_t st);              // conv_gemm_tc_f16.cu; 1 = layer not covered
-int iss_launch_conv_tc_f16g(const ConvArgs &a, cudaStream_t st);       // conv_gemm_tc_f16g.cu; 1 = layer not covered
-int iss_launch_conv_tc_f16d(ConvArgs &a, cudaStream_t st);              // conv_gemm_tc_f16d.cu; 1 = layer not covered
-
 bool iss_conv_tc_eligible(const ConvArgs &a)
 {
     return a.wt_hi && a.wt_lo && a.wt_tiled && a.Kp > 0 && a.C % 32 == 0 && a.K % 32 == 0 && a.N % 32 == 0 && a.N >= 32;
 }
 
-int iss_launch_conv_tc(const ConvArgs &a_in, int mode, cudaStream_t st)
+// n-tile width of engine 3: 128 output channels per CTA when N allows it, else 64
+int iss_f16_bn_for(int N) { return N % 128 == 0 ? 128 : 64; }
+
+bool iss_conv_f16_covers(const ConvArgs &a)
 {
-    ConvArgs a = a_in;
-    if (mode == ISS_GEMM_TC_F16) {                                      // fp16-split kernels where they apply: direct, slab, then gather
-        int rc = iss_launch_conv_tc_f16d(a, st);
-        if (rc != 1) return rc;
-        rc = iss_launch_conv_tc_f16(a, st);
-        if (rc != 1) return rc;
-        static const bool gather_off = [] { const char *e = getenv("ISS_B200_F16_GATHER"); return e && e[0] == '0'; }();   // A/B experiments
-        if (!gather_off || a.in_packed || a.out_packed || a.residual_packed) {
-            rc = iss_launch_conv_tc_f16g(a, st);
-            if (rc != 1) return rc;
-        }
-    }
-    ISS_REQUIRE(!a.in_packed && !a.out_packed && !a.residual_packed, ISS_ERR_UNSUPPORTED, "conv_tc: split-half tensors need the fp16-split engine");
-    // two accumulators per tile (main + correction) => BN <= 128 (2 x 128 + A ring <= 512 TMEM columns)
-    if (a.N % 128 == 0) return launch_tc2<128, 4, 4, 4>(a, st);          // 193 KB smem, 512 TMEM cols (2x128 acc + 4 A stages), 1 CTA/SM
-    if (a.N % 64 == 0) return launch_tc2<64, 3, 3, 2>(a, st);            //  97 KB smem, 256 TMEM cols, 2 CTAs/SM
-    return launch_tc2<32, 3, 4, 3>(a, st);                                //  81 KB smem, 256 TMEM cols
+    if (!a.wt_f16 || (a.flags & ISS_F_SIGMOID)) return false;
+    if (a.C % HBK != 0 || a.N % 64 != 0 || a.K != a.KH * a.KW * a.C) return false;
+    if (a.pool_h > 0 && (a.first || !a.in_packed || a.pool_h / 2 != a.H || a.pool_w / 2 != a.W)) return false;   // 2x2 / stride-2 'valid' pooling only
+    if (a.first && (a.C != HBK || a.SH != 1 || a.SW != 1 || a.PT != 0 || a.PL != 0 || a.OH != a.H - a.KH + 1 || a.OW != a.W - a.KW + 1 ||
+                    (a.flags & ISS_F_RESIDUAL)))
+        return false;
+    return true;
+}
+
+int iss_launch_conv_tc(const ConvArgs &a, int mode, cudaStream_t st)
+{
+    if (mode == ISS_GEMM_TC_F16 && iss_conv_f16_covers(a))
+        return iss_f16_bn_for(a.N) == 128 ? launch_f16<128>(a, st) : launch_f16<64>(a, st);
+    ISS_REQUIRE(!a.in_packed && !a.out_packed && !a.residual_packed && !a.first && a.pool_h == 0, ISS_ERR_UNSUPPORTED,
+                "conv_tc: split-half tensors, folded pooling and the fused first layer need the fp16-split engine");
+    if (a.N % 128 == 0) return launch_wg<ENG_TF32, 128, LD_F32>(a, a.wt_tiled, 1.f, st);
+    if (a.N % 64 == 0) return launch_wg<ENG_TF32, 64, LD_F32>(a, a.wt_tiled, 1.f, st);
+    return launch_wg<ENG_TF32, 32, LD_F32>(a, a.wt_tiled, 1.f, st);
 }
 
 static int tc_block_n(int N) { return N % 128 == 0 ? 128 : (N % 64 == 0 ? 64 : 32); }
 
-// Host-side preparation of a layer's weights for the tensor-core path:
+// Host-side preparation of a layer's weights for engine 2:
 // W[K][N] (Keras / our blob layout) ->
-//   (1) transposed, zero-padded, split row-major [2][N][Kp]           (SS kernel), followed by
+//   (1) transposed, zero-padded, split row-major [2][N][Kp], followed by
 //   (2) the same values tiled and pre-swizzled as smem operand images
 //       [N/BN][Kp/32][hi|lo][BN rows x 128 B, 16-byte chunk j of row n stored at chunk j ^ (n & 7)]
-//       (TS kernel: one bulk copy per stage).
+//       (one cp.async stage per k-block).
 int iss_prepare_tc_weights(const float *h_w, int K, int N, float **d_out, int *Kp_out)
 {
     const int Kp = (K + TBK - 1) / TBK * TBK;
@@ -433,5 +444,26 @@ int iss_prepare_tc_weights(const float *h_w, int K, int N, float **d_out, int *K
     if (e != cudaSuccess) { cudaFree(d); iss_set_error("cudaMemcpy tc weights: %s", cudaGetErrorString(e)); return ISS_ERR_CUDA; }
     *d_out = d;
     *Kp_out = Kp;
+    return ISS_OK;
+}
+
+// Host-side preparation of a layer's weights for engine 3: W[K][N] (Keras / blob layout) -> device image
+// [n-tile][k-block of 64][hi | lo][BN rows x 128 B, SWIZZLE_128B] of fp16 halves, pre-scaled by a power of two
+// (undone in the epilogue with *inv_scale).  Owned by the layer (freed with cudaFree by its destructor).
+int iss_prepare_f16_weights(const float *h_w, int K, int N, void **d_out, float *inv_scale)
+{
+    *d_out = nullptr; *inv_scale = 1.f;
+    if (K % HBK != 0 || N % 64 != 0) return ISS_OK;             // not a shape this engine takes
+    std::vector<float> wt((size_t)N * K, 0.f);                   // transposed [N][K]
+    for (int k = 0; k < K; ++k)
+        for (int n = 0; n < N; ++n) wt[(size_t)n * K + k] = h_w[(size_t)k * N + n];
+    std::vector<__half> img;
+    const float scale = iss_f16_build_image(wt.data(), N, K, K, iss_f16_bn_for(N), img);
+    void *d = nullptr;
+    cudaError_t e = cudaMalloc(&d, img.size() * sizeof(__half));
+    if (e != cudaSuccess) { iss_set_error("cudaMalloc f16 weights: %s", cudaGetErrorString(e)); return ISS_ERR_NOMEM; }
+    e = cudaMemcpy(d, img.data(), img.size() * sizeof(__half), cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) { cudaFree(d); iss_set_error("cudaMemcpy f16 weights: %s", cudaGetErrorString(e)); return ISS_ERR_CUDA; }
+    *d_out = d; *inv_scale = 1.f / scale;
     return ISS_OK;
 }

@@ -1,4 +1,4 @@
-// f16_image.cuh -- host-only: fp32 weights [N][Kp] -> the tiled fp16 hi/lo operand image of conv_gemm_tc_f16.cu.
+// f16_image.cuh -- host-only: fp32 weights [N][Kp] -> the tiled fp16 hi/lo operand image of engine 3 (conv_gemm_tc.cu).
 // Kept free of CUDA runtime calls so that tools/f16_image_check.cu can exercise it on a machine without a GPU.
 #pragma once
 #include <cuda_fp16.h>

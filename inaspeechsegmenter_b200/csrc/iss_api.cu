@@ -50,9 +50,9 @@ extern "C" int iss_ctx_create(int device, iss_ctx **out)
     ISS_REQUIRE(device >= 0 && device < n, ISS_ERR_INVALID, "iss_ctx_create: device %d of %d", device, n);
     cudaDeviceProp prop;
     ISS_CUDA_OK(cudaGetDeviceProperties(&prop, device));
-    // The library is compiled for sm_100a only: no PTX fallback, no other arch.
-    ISS_REQUIRE(prop.major == 10, ISS_ERR_CUDA,
-                "iss_ctx_create: device %d is sm_%d%d; libiss_b200 holds sm_100a code only",
+    // The library is compiled for sm_90a only: no PTX fallback, no other arch.
+    ISS_REQUIRE(prop.major == 9 && prop.minor == 0, ISS_ERR_CUDA,
+                "iss_ctx_create: device %d is sm_%d%d; libiss_b200 holds sm_90a code only",
                 device, prop.major, prop.minor);
     ISS_CUDA_OK(cudaSetDevice(device));
     iss_ctx *c = new iss_ctx();

@@ -1,4 +1,4 @@
-// iss_common.cuh -- shared declarations of libiss_b200 (sm_100a only).
+// iss_common.cuh -- shared declarations of libiss_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -191,10 +191,8 @@ extern "C" int iss_resnet_create(iss_ctx *ctx, const float *h_blob, int64_t blob
         const int K = c.kh * c.kw * c.cin;
         if (c.cin % 32 != 0 || K % 32 != 0 || c.cout % 32 != 0) return ISS_OK;
         const int rc = iss_prepare_tc_weights(h_blob + c.w_off, K, c.cout, &c.d_wt, &c.Kp);
-        // fp16-split image: 64-channel k-blocks; a 1x1 convolution over 32 channels is padded to one block (direct kernel only)
-        // (and one with 32 outputs to one n-tile)
-        const bool one = c.kh * c.kw == 1;
-        if (rc != ISS_OK || (c.cin % 64 != 0 && !(c.cin == 32 && one)) || (c.cout % 64 != 0 && !(c.cout == 32 && one))) return rc;
+        // fp16-split image: 64-channel k-blocks, 64-wide n-tiles
+        if (rc != ISS_OK || c.cin % 64 != 0 || c.cout % 64 != 0) return rc;
         return iss_prepare_f16_weights(h_blob + c.w_off, K, c.cout, &c.d_wt_f16, &c.f16_inv_scale);
     };
     int prc = ISS_OK;
@@ -283,15 +281,7 @@ extern "C" int iss_resnet_embed(iss_ctx *ctx, iss_resnet *net, const float *d_fe
     // Activation formats (conv_gemm.cuh): a tensor is stored as split-half words when its producer AND every consumer run on
     // the fp16-split engine (all convolutions with cin % 64 == 0 and cout % 64 == 0, i.e. stages 2-4), fp32 otherwise.
     const bool f16_mode = iss_get_gemm_mode() == ISS_GEMM_TC_F16;
-    // (a 32-channel 1x1 convolution has an image only the direct kernel reads: it counts when that kernel takes the layer)
-    auto f16 = [&](const RConv &c) {
-        if (!f16_mode || c.d_wt_f16 == nullptr) return false;
-        if (c.cin % 64 == 0 && c.cout % 64 == 0) return true;
-        ConvArgs pr = {};
-        pr.wt_f16 = c.d_wt_f16; pr.M = 1024; pr.N = c.cout; pr.K = c.kh * c.kw * c.cin; pr.Kp = c.Kp; pr.H = 32; pr.W = 32; pr.C = c.cin; pr.OH = 32; pr.OW = 32;
-        pr.KH = c.kh; pr.KW = c.kw; pr.SH = c.stride; pr.SW = c.stride; pr.PT = c.pad; pr.PL = c.pad;
-        return iss_conv_f16_direct_covers(pr);
-    };
+    auto f16 = [&](const RConv &c) { return f16_mode && c.d_wt_f16 != nullptr && c.cin % 64 == 0 && c.cout % 64 == 0; };
     auto conv = [&](const RConv &c, const float *in, bool in_packed, float *out, bool out_packed, int nb, int h, int w, int oh, int ow,
                     int flags, const float *residual, bool residual_packed) -> int {
         ConvArgs a = {};

@@ -20,7 +20,7 @@ class Context:
 
     def __init__(self, device=0):
         if not torch.cuda.is_available():
-            raise _lib.IssError('inaspeechsegmenter_b200 needs a CUDA device (B200, sm_100a); there is no CPU path')
+            raise _lib.IssError('inaspeechsegmenter_b200 needs a CUDA device (H100, sm_90a); there is no CPU path')
         self.device = torch.device('cuda', device if isinstance(device, int) else torch.device(device).index or 0)
         lib = _lib.load()
         h = ctypes.c_void_p()

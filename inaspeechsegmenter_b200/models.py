@@ -203,7 +203,7 @@ def lower_keras_model(config, weights, in_h, in_w, allow_no_head=False):
             flat = True                     # NHWC memory order == Keras channels_last flatten order
             cur = None
         else:
-            raise NotImplementedError('Keras layer %s is not supported by the B200 CNN operator' % cls)
+            raise NotImplementedError('Keras layer %s is not supported by the GPU CNN operator' % cls)
     if any(d is not descs[-1] for d in softmax_layers):
         raise NotImplementedError('softmax on a layer that is not the head')
     if not (h == 1 and w == 1) and not (allow_no_head and flat):

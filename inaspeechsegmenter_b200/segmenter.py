@@ -1,5 +1,5 @@
 """``Segmenter`` -- same public API as the reference (inaSpeechSegmenter/
-segmenter.py:207-335) with the per-frame hot path running as sm_100a CUDA
+segmenter.py:207-335) with the per-frame hot path running as sm_90a CUDA
 kernels behind the C ABI of libiss_b200.so:
 
   _media2feats   (:53-67)   -> K1 fused log-mel/log-energy kernel

@@ -1,4 +1,4 @@
-"""VBx x-vector path on B200: host mirror of the numeric part of the reference's
+"""VBx x-vector path on the GPU: host mirror of the numeric part of the reference's
 ``vbx_segmenter.py`` (constants :21-25, ``get_features`` :72-89, the
 ``VBxExtractor`` plugin ABC :205-246 and a backend :249-266).
 
@@ -303,14 +303,14 @@ def get_femininity_score(g_preds):
 
 class VoiceFemininityScoring:
     """Same contract as the reference class (vbx_segmenter.py:92-202): ``__call__(fpath) ->
-    (score, speech_duration, nb_vectors)``.  VAD = the B200 ``Segmenter('smn', detect_gender=False)``,
+    (score, speech_duration, nb_vectors)``.  VAD = this package's ``Segmenter('smn', detect_gender=False)``,
     x-vectors = K4 + K5, the gender MLP runs on device through ``iss_mlp_forward``; the interval
     bookkeeping the reference delegates to pyannote.core is plain Python here.
     Extra optional arguments: ``device``, ``ffmpeg`` and ``models`` = {'vad': (config, weights),
     'mlp': (config, weights), 'resnet': state_dict} to bypass the model-file lookup."""
 
     def __init__(self, gd_model_criteria="bgc", backend='onnx', device=0, ffmpeg='ffmpeg', models=None):
-        assert backend in ['onnx', 'b200'], "Backend should be 'onnx' (served by the B200 extractor) or 'b200'."
+        assert backend in ['onnx', 'b200'], "Backend should be 'onnx' (served by the GPU extractor) or 'b200'."
         from .engine import MlpModel
         from .models import find_model_file, load_model_file
         from .segmenter import Segmenter

@@ -1,4 +1,4 @@
-/* iss_b200.h -- C ABI of libiss_b200.so: the B200 (sm_100a) implementation of
+/* iss_b200.h -- C ABI of libiss_b200.so: the H100 (sm_90a) implementation of
  * inaSpeechSegmenter's per-frame hot path.
  *
  * The reference (ina-foss/inaSpeechSegmenter) is pure Python and has no FFI;
@@ -51,9 +51,9 @@ int iss_ctx_destroy(iss_ctx *ctx);
  * contexts); bench.py reports the delta over its timed region. */
 int64_t iss_launch_count(void);
 /* GEMM engine used by the conv / dense layers of K2 and K5 (process-wide):
- * 0 = fp32 CUDA cores; 2 = tcgen05 3xTF32 (activation operand in tensor memory) for every
- * layer shape; 3 (default) = fp16 hi/lo split on tcgen05 kind::f16 for the un-padded stride-1
- * convolutions of the segmenter CNNs, engine 2 for every other layer.  All are sm_100a code
+ * 0 = fp32 CUDA cores; 2 = 3xTF32 split on wgmma (tf32) for every layer with C, K and N
+ * multiples of 32; 3 (default) = fp16 hi/lo split on wgmma (f16) for layers with C and N
+ * multiples of 64, engine 2 for every other layer.  All are sm_90a code
  * paths of this library with fp32-class accuracy (<= 1e-5 on the softmax against the fp32
  * oracle); the default can be overridden with ISS_B200_GEMM=fp32|tc_ts|tc_f16. */
 int iss_set_gemm_mode(int mode);

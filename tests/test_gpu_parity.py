@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on the B200 box): every CUDA kernel, called
+"""GPU parity tests (run with -m gpu on an H100): every CUDA kernel, called
 through the C ABI, against the CPU oracle on the same seeded inputs and against
 the committed reference goldens.  Nothing here reads /root/reference."""
 import json
@@ -235,7 +235,7 @@ def test_k2_cnn_softmax_vs_oracle(rt, synth_models, which, nmel):
 
 @pytest.mark.parametrize('mode', [0, 2, 3])
 def test_k2_all_gemm_engines_vs_oracle(rt, synth_models, mode):
-    """fp32 CUDA-core kernel, tcgen05 3xTF32 and the default fp16-split tcgen05 engine against the fp32 oracle (1e-4)."""
+    """fp32 CUDA-core kernel, wgmma 3xTF32 and the default fp16-split wgmma engine against the fp32 oracle (1e-4)."""
     from oracle import sidekit_oracle as sk
     lib = rt['lib'].load()
     prev = lib.iss_get_gemm_mode()
@@ -257,7 +257,7 @@ def test_k2_all_gemm_engines_vs_oracle(rt, synth_models, mode):
 
 
 def test_k2_first_layer_fused_vs_standalone_and_fallback(rt, synth_models, monkeypatch):
-    """The first layer evaluated inside the second convolution's slab fill (float64 map Y, FirstFuse) against the
+    """The first layer evaluated inside the second convolution's operand fill (float64 map Y, FirstFuse) against the
     stand-alone first-layer kernel and the oracle; a batch whose patches are far apart must take the un-fused path
     (the map would not fit) and still be right."""
     from oracle import sidekit_oracle as sk
@@ -287,9 +287,9 @@ def test_k2_first_layer_fused_vs_standalone_and_fallback(rt, synth_models, monke
 
 @pytest.mark.parametrize('which,nmel', [('smn', 21), ('gender', 24)])
 def test_k2_direct_kernel_variants_vs_oracle(rt, synth_models, monkeypatch, which, nmel):
-    """The direct convolution kernel (both tcgen05 operands from shared memory: fused first layer, 2x2 max-pooling folded
-    into the slab fill) against its fall-backs -- pooling as its own kernel, the TMEM-operand slab kernel -- and the
-    oracle, on ranges that make tiles straddle patches and end in a partial tile."""
+    """The fp16-split engine with the 2x2 max-pooling folded into its operand fill against its fall-backs -- pooling as its
+    own kernel, and the 3xTF32 engine (fp32 activations, nothing folded) -- and the oracle, on ranges that make tiles
+    straddle patches and end in a partial tile."""
     from oracle import sidekit_oracle as sk
     cfg, w = synth_models[which]
     sig = synth_audio(100, seed=9).astype(np.float32) / np.float32(32768)
@@ -298,25 +298,28 @@ def test_k2_direct_kernel_variants_vs_oracle(rt, synth_models, monkeypatch, whic
     net = rt['engine'].CnnModel.from_keras(rt['ctx'], cfg, w, nmel)
     dm = torch.from_numpy(mspec).cuda()
     lib = rt['lib'].load()
+    prev = lib.iss_get_gemm_mode()
     ranges = [(0, 1), (5, 612), (700, P)]
     ref = _oracle_probs(cfg, w, mspec, nmel, ranges)
     out, launches = {}, {}
-    for name, env in (('direct', {}), ('pool_kernel', {'ISS_B200_FUSE_POOL': '0'}), ('tmem_operand', {'ISS_B200_F16_DIRECT': '0'})):
-        for k in ('ISS_B200_FUSE_POOL', 'ISS_B200_F16_DIRECT'):
-            monkeypatch.delenv(k, raising=False)
-        for k, v in env.items():
-            monkeypatch.setenv(k, v)
-        l0 = lib.iss_launch_count()
-        out[name] = net.forward(dm, ranges).cpu().numpy()
-        launches[name] = lib.iss_launch_count() - l0
-    for k in ('ISS_B200_FUSE_POOL', 'ISS_B200_F16_DIRECT'):
-        monkeypatch.delenv(k, raising=False)
+    try:
+        for name, mode, env in (('folded', 3, {}), ('pool_kernel', 3, {'ISS_B200_FUSE_POOL': '0'}), ('engine2', 2, {})):
+            monkeypatch.delenv('ISS_B200_FUSE_POOL', raising=False)
+            for k, v in env.items():
+                monkeypatch.setenv(k, v)
+            rt['lib'].check(lib.iss_set_gemm_mode(mode), 'set mode')
+            l0 = lib.iss_launch_count()
+            out[name] = net.forward(dm, ranges).cpu().numpy()
+            launches[name] = lib.iss_launch_count() - l0
+    finally:
+        lib.iss_set_gemm_mode(prev)
+        monkeypatch.delenv('ISS_B200_FUSE_POOL', raising=False)
     for name, got in out.items():
         assert np.abs(got - ref).max() <= 1e-4, name
-    assert np.abs(out['direct'] - out['pool_kernel']).max() == 0.0          # the fused pooling keeps the same words
-    assert np.abs(out['direct'] - out['tmem_operand']).max() <= 2e-5
-    assert launches['direct'] < launches['pool_kernel']
-    REPORT['k2_direct_variants_%s' % which] = dict(vs_oracle={k: float(np.abs(v - ref).max()) for k, v in out.items()}, launches=launches)
+    assert np.abs(out['folded'] - out['pool_kernel']).max() == 0.0          # the folded pooling keeps the same words
+    assert np.abs(out['folded'] - out['engine2']).max() <= 2e-5
+    assert launches['folded'] < launches['pool_kernel']
+    REPORT['k2_folded_pooling_%s' % which] = dict(vs_oracle={k: float(np.abs(v - ref).max()) for k, v in out.items()}, launches=launches)
 
 
 @pytest.mark.parametrize('L', [68, 69, 70, 101, 135, 136])
@@ -463,7 +466,7 @@ def _alt_keras_cnn(nmel, n_classes, seed):
         L.append({'class_name': 'BatchNormalization', 'config': {'name': name, 'axis': -1, 'epsilon': 1e-3, 'center': True, 'scale': scale}})
 
     L.append({'class_name': 'InputLayer', 'config': {'name': 'in', 'batch_input_shape': [None, 68, nmel, 1]}})
-    conv('c1', 3, 3, 1, 32, [1, 1], 'same', 'relu')                       # first layer with padding (direct kernel, padded)
+    conv('c1', 3, 3, 1, 32, [1, 1], 'same', 'relu')                       # first layer with padding (first-layer kernel, padded)
     conv('c2', 3, 3, 32, 64, [2, 1], 'same', 'linear', bias=False)        # stride 2 in time, asymmetric 'same' padding, TC path
     bn('b2', 64, scale=False)
     L.append({'class_name': 'Activation', 'config': {'name': 'a2', 'activation': 'relu'}})

@@ -228,8 +228,8 @@ sys.stdout.buffer.write(hdr + b'data' + struct.pack('<I', 0xFFFFFFFF) + pcm)
 
 
 def test_kernel_source_stamp_ignores_comments_only():
-    """bench.py quotes roofline.traffic from a committed ncu summary only when the summary's stamp equals the hash of the
-    kernel's CODE: comments and white space must not change the stamp, code must."""
+    """A profile summary is stamped with the hash of the dominant kernel's CODE, so that it can be matched to the sources it
+    was captured from: comments and white space must not change the stamp, code must."""
     import bench
     a = 'int f(int x) { return x + 1; }  // adds one\n/* block\n   comment */ const char *s = "a // b /* c */";\n'
     b = 'int f(int x)\n{\n    return x + 1;\n}\nconst char *s = "a // b /* c */";   // moved\n'

@@ -1,6 +1,6 @@
 """CPU: numerical design check of the operand-split schemes the tensor-core GEMM can use.
 
-The tcgen05 path evaluates fp32 layers as sums of low-precision products (DESIGN.md 4.1/4.2).  This
+The tensor-core path evaluates fp32 layers as sums of low-precision products (DESIGN.md).  This
 emulates the schemes on the stand-in VAD network in float64 (exact products, exact accumulation -- i.e.
 the algorithmic error of the split alone, without the tensor core's truncating accumulate) and checks
 them against the fp32 oracle with the north-star tolerance (1e-4 on the per-frame softmax):

@@ -1,108 +1,97 @@
-"""CPU model of the residual-box ring of the direct kernel's TMA mode (csrc/conv_gemm_tc_f16d.cu).  The producer warp
-walks a cursor (tile, pass, 32-channel half, sub-tile); each group of four epilogue warps owns one half of the ring and
-derives (slot, phase) of its k-th box from its own loop counters.  Both sides must agree on (slot, phase, tensor
-coordinates) for every tiling the host can choose, every slot must have exactly one consumer group and its phases must
-advance one at a time, or the mbarrier parities drift and the kernel reads the wrong box."""
+"""CPU model of the shared-memory pipeline of the wgmma convolution kernel (csrc/conv_gemm_tc.cu, conv_gemm_wg_kernel).
+
+Two warpgroups run the same k-block loop.  Per k-block kb each one
+  fills its operand tile A[g][kb % 2]                    (st.shared; the tile was read by its own wgmmas of kb - 2),
+  waits for the weight stage of kb                        (cp.async.wait_group 1: only the newest commit group may pend),
+  meets the other warpgroup at __syncthreads,
+  copies its share of the weights of kb + 2 into stage (kb + 2) % B_STAGES and commits a group (empty past the end),
+  issues its wgmmas of kb on A[g][kb % 2] and stage kb % B_STAGES, then wgmma.wait_group 1 (its kb - 1 retires).
+The weights of k-blocks 0 and 1 are copied before the loop.  A wgmma may retire at any moment after it is issued and
+must have retired when wait_group says so.  Both sides must agree on the stage of every k-block, the commit groups must
+make the weights of kb complete at its wait, and no tile or stage may be overwritten while a wgmma that reads it can
+still be in flight -- for every interleaving of the two warpgroups."""
 import itertools
+import random
 
-DBN = 64
-
-
-def producer_boxes(n_tiles, grid, block, N, M, DT, rs):
-    """(slot, use, c0, row0) in issue order (Cur / advance / box_of + the slot rule of the producer loop)."""
-    nt_total = (N + DBN - 1) // DBN
-    half = rs >> 1
-    tile, nt, c, t = block, 0, 0, 0
-    out, ck = [], 0
-    more = tile < n_tiles
-    while more:
-        grp = t if DT == 2 else c >> 5
-        k = ck if DT == 2 else ck >> 1
-        row0 = tile * (DT * 128) + t * 128
-        out.append((grp * half + k % half, k // half, nt * DBN + c, row0 if row0 < M else 0))
-        if t == DT - 1:
-            ck += 1
-        ncol = min(DBN, N - nt * DBN)                                # advance
-        t += 1
-        if t < DT:
-            continue
-        t = 0
-        c += 32
-        if c < ncol:
-            continue
-        c = 0
-        nt += 1
-        if nt < nt_total:
-            continue
-        nt = 0
-        tile += grid
-        more = tile < n_tiles
-    return out
+B_STAGES, A_STAGES, AHEAD = 4, 2, 2
 
 
-def consumer_boxes(n_tiles, grid, block, N, M, DT, rs):
-    """per group: [(slot, use, c0, row0)] in the order its four warps wait for them."""
-    nt_total = (N + DBN - 1) // DBN
-    half = rs >> 1
-    seq = {0: [], 1: []}
-    for egrp in (0, 1):
-        chunk = 0
-        for tile in range(block, n_tiles, grid):
-            for nt in range(nt_total):
-                nb = nt * DBN
-                ncol = min(DBN, N - nb)
-                split_t, split_c = DT == 2, DT == 1                   # (8 epilogue warps)
-                t_first = egrp if split_t else 0
-                t_last = t_first + 1 if split_t else DT
-                c_first, c_step = (32 * egrp, 64) if split_c else (0, 32)
-                for t in range(t_first, t_last):
-                    row0 = tile * (DT * 128) + t * 128
-                    for c in range(c_first, ncol, c_step):
-                        ck = chunk + (c >> 5)
-                        k = ck if DT == 2 else ck >> 1
-                        seq[egrp].append((egrp * half + k % half, k // half, nb + c, row0 if row0 < M else 0))
-                chunk += ncol >> 5
-    return seq
+def weight_schedule(nkb, stages=B_STAGES):
+    """(k-block, stage) written by each commit group, in commit order; None = empty group."""
+    groups = [(kb, kb % stages) if kb < nkb else None for kb in range(AHEAD)]
+    for kb in range(nkb):
+        nxt = kb + AHEAD
+        groups.append((nxt, nxt % stages) if nxt < nkb else None)
+    return groups
 
 
 def test_producer_and_consumers_agree_on_every_box():
-    for DT, N, n_tiles, grid, rs in itertools.product((1, 2), (64, 128, 512), (1, 5, 9), (1, 4), (2, 4)):
-        M = n_tiles * DT * 128 - 70                                   # the last sub-tile is partly behind the last row
-        if DT == 2 and n_tiles > 1:
-            M = (n_tiles - 1) * 256 + 100                             # ... or wholly behind it (t = 1 of the last tile)
-        half = rs >> 1
-        for block in range(min(grid, n_tiles)):
-            prod = producer_boxes(n_tiles, grid, block, N, M, DT, rs)
-            cons = consumer_boxes(n_tiles, grid, block, N, M, DT, rs)
-            for grp in (0, 1):
-                mine = [b for b in prod if b[0] // half == grp]       # the producer's boxes in this group's half of the ring
-                assert mine == cons[grp], (DT, N, n_tiles, grid, rs, block, grp)
-            assert len(prod) == len(cons[0]) + len(cons[1])
-            # per slot the phases advance one at a time, starting at 0
-            for slot in range(rs):
-                uses = [b[1] for b in prod if b[0] == slot]
-                assert uses == list(range(len(uses))), (DT, N, rs, slot)
+    for nkb in range(1, 40):
+        groups = weight_schedule(nkb)
+        written = {g[0]: g[1] for g in groups if g is not None}
+        assert sorted(written) == list(range(nkb))
+        for kb in range(nkb):
+            assert written[kb] == kb % B_STAGES                       # the stage the wgmmas of kb read
+            # at the wait of iteration kb the groups committed so far are the prologue's and those of iterations < kb;
+            # wait_group 1 lets only the newest pend, so the group of kb must not be the newest
+            committed = AHEAD + kb
+            idx = next(i for i, g in enumerate(groups) if g is not None and g[0] == kb)
+            assert idx < committed - 1, (nkb, kb)
+
+
+def run(nkb, stages, rng):
+    """One random interleaving of the two warpgroups; returns the hazards seen (empty when the pipeline is safe)."""
+    steps = ['fill', 'wait', 'bar', 'copy', 'mma']
+    pc = [[0, 0], [0, 0]]                                           # (k-block, step) per warpgroup
+    inflight = [set(), set()]                                       # k-blocks whose wgmmas may still run
+    at_bar = [False, False]
+    hazards = []
+    while any(p[0] < nkb for p in pc):
+        for g in (0, 1):                                            # a wgmma may retire at any time
+            for k in list(inflight[g]):
+                if rng.random() < 0.3:
+                    inflight[g].discard(k)
+        movable = [g for g in (0, 1) if pc[g][0] < nkb and not at_bar[g]]
+        if not movable:
+            if all(at_bar[g] or pc[g][0] >= nkb for g in (0, 1)):
+                for g in (0, 1):
+                    if at_bar[g]:
+                        at_bar[g] = False
+                        pc[g][1] += 1
+                continue
+            raise AssertionError('deadlock')
+        g = rng.choice(movable)
+        kb, st = pc[g]
+        step = steps[st]
+        if step == 'fill':
+            if any(k % A_STAGES == kb % A_STAGES for k in inflight[g]):
+                hazards.append(('A', g, kb))
+        elif step == 'bar':
+            at_bar[g] = True
+            if all(at_bar[h] or pc[h][0] >= nkb for h in (0, 1)):
+                for h in (0, 1):
+                    if at_bar[h]:
+                        at_bar[h] = False
+                        pc[h][1] += 1
+            continue
+        elif step == 'copy':
+            nxt = kb + AHEAD
+            if nxt < nkb and any(k % stages == nxt % stages for h in (0, 1) for k in inflight[h]):
+                hazards.append(('B', g, nxt))
+        elif step == 'mma':
+            inflight[g].add(kb)
+            inflight[g] = {k for k in inflight[g] if k >= kb}          # wait_group 1: only the group just committed may pend
+        pc[g][1] += 1
+        if pc[g][1] == len(steps):
+            pc[g] = [kb + 1, 0]
+    return hazards
 
 
 def test_ring_never_deadlocks():
-    """The producer refills a slot only after its previous box has been released; the two groups advance independently.
-    Simulate the slowest legal interleaving and check that everything drains."""
-    for DT, N, rs in itertools.product((1, 2), (64, 512), (2, 4)):
-        n_tiles, grid, block = 6, 2, 1
-        M = n_tiles * DT * 128
-        prod = producer_boxes(n_tiles, grid, block, N, M, DT, rs)
-        cons = consumer_boxes(n_tiles, grid, block, N, M, DT, rs)
-        queues = {e: list(cons[e]) for e in (0, 1)}
-        loaded, released, issued = set(), set(), 0
-        progress = True
-        while progress:
-            progress = False
-            while issued < len(prod):
-                slot, use = prod[issued][:2]
-                if use > 0 and (slot, use - 1) not in released:
-                    break
-                loaded.add((slot, use)); issued += 1; progress = True
-            for e in (0, 1):
-                if queues[e] and queues[e][0][:2] in loaded:
-                    released.add(queues[e].pop(0)[:2]); progress = True
-        assert issued == len(prod) and not queues[0] and not queues[1], (DT, N, rs)
+    """Random interleavings (seeded) of the two warpgroups drain without deadlock and without a hazard.  With three weight
+    stages instead of four the copy of kb + 2 would land on the stage the other warpgroup may still be reading for
+    kb - 1: the model finds that hazard, which is why the ring has four stages at this prefetch distance."""
+    rng = random.Random(20261015)
+    for nkb, _ in itertools.product((1, 2, 3, 5, 9, 20), range(60)):
+        assert run(nkb, B_STAGES, rng) == [], nkb
+    assert any(run(9, 3, rng) for _ in range(200))

@@ -1,5 +1,5 @@
 // f16_image_check.cu -- host-only check of iss_f16_build_image (runs without a GPU):
-//   * an independent reader that follows the UMMA shared-memory descriptor semantics (K-major, SWIZZLE_128B:
+//   * an independent reader that follows the wgmma shared-memory descriptor semantics (K-major, SWIZZLE_128B:
 //     row r of a tile at byte r*128, 16-byte chunk c of that row at chunk c ^ (r & 7)) recovers B[n][k];
 //   * (hi + lo) / scale reproduces every weight to 2^-21 relative or 2^-36 of the layer maximum (the fp16 subnormal floor after scaling);
 //   * the scaled maximum lies in [2^12, 2^13).

@@ -25,7 +25,7 @@ def rep_summary(path):
     rows = list(csv.reader(io.StringIO(raw)))
     hdr, units = rows[0], rows[1]
     out = ['# %s  (ncu --set full --clock-control none; per launch, cold cache, serialised)' % path]
-    try:                                   # stamp: bench.py only quotes `traffic` from a summary captured from the current kernel sources
+    try:                                   # stamp: which kernel sources the summary was captured from (bench.kernel_source_hash)
         import os
         sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
         from bench import kernel_source_hash

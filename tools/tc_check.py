@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Bring-up check of the tcgen05 GEMM modes: run the VAD stand-in CNN on synthetic
+"""Bring-up check of the GEMM engines: run the VAD stand-in CNN on synthetic
 log-mel with one GEMM mode, compare with the fp32 CUDA-core result saved by mode 0,
 and time a larger batch.  Each mode runs in its own process (a hung kernel must not
 take the others down):  python tools/tc_check.py <mode 0|2|3> [minutes]
