@@ -29,6 +29,10 @@
 // memory operand image ([n-tile][k-block][hi|lo][BN rows x 128 B]); all 256 threads copy a stage with cp.async, four
 // stages deep (two k-blocks ahead).  The global loads of k-block kb+1 are in flight while the wgmmas of kb are issued,
 // and wgmma.wait_group 1 keeps one k-block of tensor work running while the next tile is filled.
+//
+// The un-padded, stride-1 64 -> 64 convolutions of engine 3 (the segmenter CNNs' dominant 5x4 layer, with or without the
+// fused first layer) run in conv_slab_kernel instead: it fills each input value once per tile into a "slab" whose
+// row-shifted windows are the A operands of all taps, where the gather kernel above fills it once per tap.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <stdio.h>
@@ -49,8 +53,8 @@ constexpr int A_WG = 16384;                  // one warpgroup's operand tile of 
 constexpr int A_STAGES = 2, B_STAGES = 4;
 
 constexpr int ENG_TF32 = 0, ENG_F16 = 1;
-// operand fill of engine 3: fp32 values split here, split-half words, words with the 2x2 max-pooling in front, or the
-// fused first layer.  Engine 2 reads fp32 values only.
+// operand fill of engine 3: fp32 values split here, split-half words, words with the 2x2 max-pooling in front (gather
+// kernel only), or the fused first layer (slab kernel only).  Engine 2 reads fp32 values only.
 constexpr int LD_F32 = 0, LD_PACKED = 1, LD_POOL = 2, LD_FIRST = 3;
 
 template <int BN>
@@ -80,9 +84,59 @@ __device__ __forceinline__ void words_to_planes(const uint32_t (&w)[8], uint32_t
     }
 }
 
+// Epilogue of both kernels for the output pair (m, nb), (m, nb + 1): inv_scale (engine 3), bias, pre-affine, residual,
+// ReLU, post-affine, then fp32 values or split-half words.
+struct EpiCoef {
+    float eb[2], es1[2], et1[2], es2[2], et2[2];
+};
+
+__device__ __forceinline__ EpiCoef epi_coef(const ConvArgs &a, int nb)
+{
+    const bool has_bias = a.flags & ISS_F_BIAS, pre = a.flags & ISS_F_AFFINE_PRE, post = a.flags & ISS_F_AFFINE_POST;
+    EpiCoef c;
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+        c.eb[q] = has_bias ? __ldg(a.bias + nb + q) : 0.f;
+        c.es1[q] = pre ? __ldg(a.pre_scale + nb + q) : 1.f;  c.et1[q] = pre ? __ldg(a.pre_shift + nb + q) : 0.f;
+        c.es2[q] = post ? __ldg(a.post_scale + nb + q) : 1.f; c.et2[q] = post ? __ldg(a.post_shift + nb + q) : 0.f;
+    }
+    return c;
+}
+
+template <int ENG>
+__device__ __forceinline__ void epi_store(const ConvArgs &a, const EpiCoef &c, int64_t m, int nb, float y0, float y1, float inv_scale)
+{
+    const bool pre = a.flags & ISS_F_AFFINE_PRE, post = a.flags & ISS_F_AFFINE_POST;
+    const bool relu = a.flags & ISS_F_RELU, resid = a.flags & ISS_F_RESIDUAL;
+    float y[2] = {y0, y1};
+    float rv[2] = {0.f, 0.f};
+    if (resid) {
+        const uint2 rw = __ldg(reinterpret_cast<const uint2 *>(a.residual + m * a.N + nb));
+        if (a.residual_packed) { rv[0] = iss_unpack_split(rw.x); rv[1] = iss_unpack_split(rw.y); }
+        else { rv[0] = __uint_as_float(rw.x); rv[1] = __uint_as_float(rw.y); }
+    }
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+        float v;
+        if constexpr (ENG == ENG_F16)                         // ((acc * inv_s) + bias) * s1 + t1 as one multiply-add
+            v = fmaf(y[q], inv_scale * c.es1[q], fmaf(c.eb[q], c.es1[q], c.et1[q]));
+        else {
+            v = y[q] + c.eb[q];
+            if (pre) v = fmaf(v, c.es1[q], c.et1[q]);
+        }
+        if (resid) v += rv[q];
+        if (relu) v = fmaxf(v, 0.f);
+        if (post) v = fmaf(v, c.es2[q], c.et2[q]);
+        y[q] = v;
+    }
+    float *dst = a.out + m * a.N + nb;
+    if (a.out_packed) *reinterpret_cast<uint2 *>(dst) = make_uint2(iss_pack_split(y[0]), iss_pack_split(y[1]));
+    else *reinterpret_cast<float2 *>(dst) = make_float2(y[0], y[1]);
+}
+
 template <int ENG, int BN, int MODE>
 __global__ void __launch_bounds__(THREADS, 1)
-conv_gemm_wg_kernel(const ConvArgs a, const FirstFuse ff, const unsigned char *__restrict__ wt, float inv_scale)
+conv_gemm_wg_kernel(const ConvArgs a, const unsigned char *__restrict__ wt, float inv_scale)
 {
     using Cfg = WgCfg<BN>;
     constexpr int KE = ENG == ENG_F16 ? HBK : TBK;                       // k-elements per block
@@ -181,7 +235,8 @@ conv_gemm_wg_kernel(const ConvArgs a, const FirstFuse ff, const unsigned char *_
             } else if constexpr (MODE == LD_PACKED) {
                 const uint32_t w[8] = {raw[i][0].x, raw[i][0].y, raw[i][0].z, raw[i][0].w, raw[i][1].x, raw[i][1].y, raw[i][1].z, raw[i][1].w};
                 words_to_planes(w, hw, lw);
-            } else if constexpr (MODE == LD_POOL) {
+            } else {
+                static_assert(MODE == LD_POOL, "the fused first layer runs in conv_slab_kernel");
                 // the 2x2 window of the un-pooled NHWC tensor [img][pool_h][pool_w][C]: the WORD of the largest value is kept
                 // (as maxpool_nhwc_packed_kernel does: window order (0,0) (0,1) (1,0) (1,1), NaN wins, first maximum wins)
                 uint32_t bw[8] = {0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
@@ -204,33 +259,6 @@ conv_gemm_wg_kernel(const ConvArgs a, const FirstFuse ff, const unsigned char *_
                     }
                 }
                 words_to_planes(bw, hw, lw);
-            } else {                                          // LD_FIRST (C = 64, stride 1, no padding)
-                float v[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-                int ih, iw;
-                if (pixel_ok(i, ih, iw)) {
-                    const int img = row_img[i];
-                    const int64_t o = (((int64_t)__ldg(ff.row0 + img) - ff.y_f0 + ih) * a.W + iw) * HBK + j * 8;
-                    const float4 *yh = reinterpret_cast<const float4 *>(ff.Yh + o), *yl = reinterpret_cast<const float4 *>(ff.Yl + o);
-                    const float4 *cf = reinterpret_cast<const float4 *>(ff.coef + (int64_t)img * (3 * HBK) + j * 8);
-#pragma unroll
-                    for (int q = 0; q < 2; ++q) {
-                        const float4 h4 = __ldg(yh + q), l4 = __ldg(yl + q);
-                        const float4 va = __ldg(cf + q), vh = __ldg(cf + HBK / 4 + q), vl = __ldg(cf + 2 * (HBK / 4) + q);
-                        const float hv[4] = {h4.x, h4.y, h4.z, h4.w}, lv[4] = {l4.x, l4.y, l4.z, l4.w};
-                        const float al[4] = {va.x, va.y, va.z, va.w}, bh[4] = {vh.x, vh.y, vh.z, vh.w}, bl[4] = {vl.x, vl.y, vl.z, vl.w};
-#pragma unroll
-                        for (int e = 0; e < 4; ++e) {
-                            float u = fmaf(hv[e], al[e], bh[e]) + fmaf(lv[e], al[e], bl[e]);
-                            if (ff.flags & ISS_F_RELU) u = fmaxf(u, 0.f);
-                            if (ff.flags & ISS_F_AFFINE_POST) {
-                                const int c = j * 8 + 4 * q + e;
-                                u = fmaf(u, __ldg(ff.post_scale + c), __ldg(ff.post_shift + c));
-                            }
-                            v[4 * q + e] = u;
-                        }
-                    }
-                }
-                split_f16(v, hw, lw);
             }
             sts128(hi_base + dst, hw[0], hw[1], hw[2], hw[3]);
             sts128(lo_base + dst, lw[0], lw[1], lw[2], lw[3]);
@@ -277,46 +305,15 @@ conv_gemm_wg_kernel(const ConvArgs a, const FirstFuse ff, const unsigned char *_
     // ============================ epilogue (from the accumulator registers) ============================
     const int w = t >> 5, l = t & 31;
     const int64_t mr = m0 + 16 * w + (l >> 2);
-    const bool has_bias = a.flags & ISS_F_BIAS, pre = a.flags & ISS_F_AFFINE_PRE, post = a.flags & ISS_F_AFFINE_POST;
-    const bool relu = a.flags & ISS_F_RELU, resid = a.flags & ISS_F_RESIDUAL;
 #pragma unroll
     for (int i = 0; i < BN / 8; ++i) {
         const int nb = n0 + 8 * i + 2 * (l & 3);
-        float eb[2], es1[2], et1[2], es2[2], et2[2];
-#pragma unroll
-        for (int q = 0; q < 2; ++q) {
-            eb[q] = has_bias ? __ldg(a.bias + nb + q) : 0.f;
-            es1[q] = pre ? __ldg(a.pre_scale + nb + q) : 1.f;  et1[q] = pre ? __ldg(a.pre_shift + nb + q) : 0.f;
-            es2[q] = post ? __ldg(a.post_scale + nb + q) : 1.f; et2[q] = post ? __ldg(a.post_shift + nb + q) : 0.f;
-        }
+        const EpiCoef c = epi_coef(a, nb);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int64_t m = mr + 8 * h;
             if (m >= a.M) continue;
-            float y[2] = {dm[4 * i + 2 * h] + dl[4 * i + 2 * h], dm[4 * i + 2 * h + 1] + dl[4 * i + 2 * h + 1]};
-            float rv[2] = {0.f, 0.f};
-            if (resid) {
-                const uint2 rw = __ldg(reinterpret_cast<const uint2 *>(a.residual + m * a.N + nb));
-                if (a.residual_packed) { rv[0] = iss_unpack_split(rw.x); rv[1] = iss_unpack_split(rw.y); }
-                else { rv[0] = __uint_as_float(rw.x); rv[1] = __uint_as_float(rw.y); }
-            }
-#pragma unroll
-            for (int q = 0; q < 2; ++q) {
-                float v;
-                if constexpr (ENG == ENG_F16)                 // ((acc * inv_s) + bias) * s1 + t1 as one multiply-add
-                    v = fmaf(y[q], inv_scale * es1[q], fmaf(eb[q], es1[q], et1[q]));
-                else {
-                    v = y[q] + eb[q];
-                    if (pre) v = fmaf(v, es1[q], et1[q]);
-                }
-                if (resid) v += rv[q];
-                if (relu) v = fmaxf(v, 0.f);
-                if (post) v = fmaf(v, es2[q], et2[q]);
-                y[q] = v;
-            }
-            float *dst = a.out + m * a.N + nb;
-            if (a.out_packed) *reinterpret_cast<uint2 *>(dst) = make_uint2(iss_pack_split(y[0]), iss_pack_split(y[1]));
-            else *reinterpret_cast<float2 *>(dst) = make_float2(y[0], y[1]);
+            epi_store<ENG>(a, c, m, nb, dm[4 * i + 2 * h] + dl[4 * i + 2 * h], dm[4 * i + 2 * h + 1] + dl[4 * i + 2 * h + 1], inv_scale);
         }
     }
 }
@@ -329,9 +326,192 @@ int launch_wg(const ConvArgs &a, const void *wt, float inv_scale, cudaStream_t s
     ISS_CUDA_OK(iss_optin_smem(reinterpret_cast<const void *>(kern), Cfg::SMEM));
     const int64_t gm = (a.M + TBM - 1) / TBM;
     ISS_REQUIRE(gm < (1ll << 31), ISS_ERR_INVALID, "conv_tc: M too large");
-    const FirstFuse ff = a.first ? *a.first : FirstFuse{};
     dim3 grid((unsigned)gm, (unsigned)(a.N / BN));
-    kern<<<grid, THREADS, Cfg::SMEM, st>>>(a, ff, reinterpret_cast<const unsigned char *>(wt), inv_scale);
+    kern<<<grid, THREADS, Cfg::SMEM, st>>>(a, reinterpret_cast<const unsigned char *>(wt), inv_scale);
+    ISS_CUDA_OK(cudaGetLastError());
+    iss_count_launch();
+    return ISS_OK;
+}
+
+// ============================ slab kernel: un-padded, stride-1 engine-3 convolutions with C = N = 64 ============================
+// The input of a batch is read as ONE tall image, pixel p = (img * H + ih) * W + iw, and every output slot gets the same
+// numbering, s = (img * H + oh) * W + ow.  The A operand of tap (kh, kw) for the slots s0 .. s0 + 63 is then the 64
+// consecutive pixels from s0 + kh * W + kw.  A CTA owns the slots s0 .. s0 + 255 (four warpgroups of 64); it evaluates,
+// splits and stores the pixels s0 .. s0 + 255 + (KH - 1) W + KW - 1 once into a SWIZZLE_128B hi plane and lo plane (the
+// "slab"), and every tap's A tile is a row-shifted window of it, addressed by the wgmma descriptor alone.  So each input
+// value is filled about 1.3 times instead of KH * KW times.  Slots with oh >= OH or ow >= OW (and slots past the batch)
+// are computed and not stored.  Slab rows past the last pixel of the batch are zero.
+// The weight stage of a tap is the engine-3 image [hi: 64 rows | lo: 64 rows] x 128 B, read as ONE 128-row B operand, so
+// Ah.[Bh | Bl] is one m64n128k16 (accumulator columns 0..63 = Ah.Bh, 64..127 = Ah.Bl) and Al.Bh one m64n64k16 into its
+// own accumulator: A is read twice per k16 step instead of three times.  (wgmma orders accumulator accesses only between
+// instructions of one shape, so the two shapes never share registers.)
+constexpr int SLAB_TS = 256, SLAB_THREADS = 512, SLAB_C = 64, SLAB_N = 64;
+constexpr int SLAB_B_STAGE = 2 * SLAB_N * 128;          // hi | lo, 64 rows x 128 B each
+constexpr int SLAB_B_STAGES = 4;
+constexpr int SLAB_MAX_SMEM = 227 * 1024;
+
+// slab rows of a tile (a multiple of 8, so that the lo plane stays 1024-byte aligned) and the kernel's shared memory
+int slab_rows(int KH, int KW, int W) { return (SLAB_TS + (KH - 1) * W + KW - 1 + 7) & ~7; }
+int slab_smem(int rows) { return SLAB_B_STAGES * SLAB_B_STAGE + 2 * rows * 128 + 1024; }
+
+template <int MODE>
+__global__ void __launch_bounds__(SLAB_THREADS, 1)
+conv_slab_kernel(const ConvArgs a, const FirstFuse ff, const unsigned char *__restrict__ wt, float inv_scale, int rows)
+{
+    extern __shared__ unsigned char smem_dyn[];
+    unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
+    const uint32_t b_ring_u32 = smem_u32(smem);
+    const uint32_t slab_hi = b_ring_u32 + SLAB_B_STAGES * SLAB_B_STAGE, slab_lo = slab_hi + (uint32_t)rows * 128u;
+
+    const int tid = threadIdx.x, wg = tid >> 7, t = tid & 127;
+    const int64_t s0 = (int64_t)blockIdx.x * SLAB_TS;
+    const int nkb = a.KH * a.KW;                             // one k-block (64 channels) per tap
+    const int64_t HW = (int64_t)a.H * a.W;
+    const int64_t n_img = a.M / ((int64_t)a.OH * a.OW);
+    const int64_t npix = n_img * HW;
+
+    auto issue_b = [&](int kb) {
+        if (kb < nkb) {
+            const unsigned char *src = wt + (size_t)kb * SLAB_B_STAGE;
+            const uint32_t dst = b_ring_u32 + (uint32_t)(kb % SLAB_B_STAGES) * SLAB_B_STAGE;
+#pragma unroll
+            for (int o = tid * 16; o < SLAB_B_STAGE; o += SLAB_THREADS * 16) cp_async16_u32(dst + o, src + o, 16);
+        }
+        cp_async_commit();                                   // (empty groups keep the group count uniform)
+    };
+    issue_b(0);
+    issue_b(1);
+
+    // ---- the slab: 16-byte chunk j of pixel row r at chunk j ^ (r & 7) of both planes ----
+#pragma unroll 2
+    for (int u = tid; u < rows * 8; u += SLAB_THREADS) {
+        const int r = u >> 3, j = u & 7;
+        const int64_t p = s0 + r;
+        uint32_t hw[4] = {0u, 0u, 0u, 0u}, lw[4] = {0u, 0u, 0u, 0u};
+        if (p < npix) {
+            if constexpr (MODE == LD_FIRST) {                 // the first layer at pixel p, from the map Y of its own patch
+                const int64_t img = p / HW;
+                const int rem = (int)(p - img * HW);
+                const int ih = rem / a.W, iw = rem - ih * a.W;
+                const int64_t o = (((int64_t)__ldg(ff.row0 + img) - ff.y_f0 + ih) * a.W + iw) * SLAB_C + j * 8;
+                const float4 *yh = reinterpret_cast<const float4 *>(ff.Yh + o), *yl = reinterpret_cast<const float4 *>(ff.Yl + o);
+                const float4 *cf = reinterpret_cast<const float4 *>(ff.coef + img * (3 * SLAB_C) + j * 8);
+                float v[8];
+#pragma unroll
+                for (int q = 0; q < 2; ++q) {
+                    const float4 h4 = __ldg(yh + q), l4 = __ldg(yl + q);
+                    const float4 va = __ldg(cf + q), vh = __ldg(cf + SLAB_C / 4 + q), vl = __ldg(cf + 2 * (SLAB_C / 4) + q);
+                    const float hv[4] = {h4.x, h4.y, h4.z, h4.w}, lv[4] = {l4.x, l4.y, l4.z, l4.w};
+                    const float al[4] = {va.x, va.y, va.z, va.w}, bh[4] = {vh.x, vh.y, vh.z, vh.w}, bl[4] = {vl.x, vl.y, vl.z, vl.w};
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) {
+                        float x = fmaf(hv[e], al[e], bh[e]) + fmaf(lv[e], al[e], bl[e]);
+                        if (ff.flags & ISS_F_RELU) x = fmaxf(x, 0.f);
+                        if (ff.flags & ISS_F_AFFINE_POST) {
+                            const int c = j * 8 + 4 * q + e;
+                            x = fmaf(x, __ldg(ff.post_scale + c), __ldg(ff.post_shift + c));
+                        }
+                        v[4 * q + e] = x;
+                    }
+                }
+                split_f16(v, hw, lw);
+            } else {                                          // NHWC pixel p of the batch is the tall image's pixel p
+                const uint4 *src = reinterpret_cast<const uint4 *>(a.in + p * SLAB_C + j * 8);
+                const uint4 u0 = __ldg(src), u1 = __ldg(src + 1);
+                if constexpr (MODE == LD_PACKED) {
+                    const uint32_t w[8] = {u0.x, u0.y, u0.z, u0.w, u1.x, u1.y, u1.z, u1.w};
+                    words_to_planes(w, hw, lw);
+                } else {
+                    static_assert(MODE == LD_F32, "slab fill modes: LD_F32, LD_PACKED, LD_FIRST");
+                    const float v[8] = {__uint_as_float(u0.x), __uint_as_float(u0.y), __uint_as_float(u0.z), __uint_as_float(u0.w),
+                                        __uint_as_float(u1.x), __uint_as_float(u1.y), __uint_as_float(u1.z), __uint_as_float(u1.w)};
+                    split_f16(v, hw, lw);
+                }
+            }
+        }
+        const uint32_t dst = (uint32_t)r * 128u + ((uint32_t)(j ^ (r & 7)) << 4);
+        sts128(slab_hi + dst, hw[0], hw[1], hw[2], hw[3]);
+        sts128(slab_lo + dst, lw[0], lw[1], lw[2], lw[3]);
+    }
+
+    float dm[SLAB_N], dl[SLAB_N / 2];                        // dm: [Ah.Bh | Ah.Bl] (n128), dl: Al.Bh (n64)
+#pragma unroll
+    for (int q = 0; q < SLAB_N; ++q) dm[q] = 0.f;
+#pragma unroll
+    for (int q = 0; q < SLAB_N / 2; ++q) dl[q] = 0.f;
+    wgmma_fence_operand(dm);                                 // keep the zeroing out of the wgmma pipeline (ptxas would
+    wgmma_fence_operand(dl);                                 // otherwise serialize every wgmma of the loop)
+
+    int kh = 0, kw = 0;
+    for (int kb = 0; kb < nkb; ++kb) {
+        cp_async_wait<1>();                                  // weights of kb landed (kb + 1 may still be in flight)
+        fence_proxy_async();                                 // (and, at kb = 0, this thread's slab stores)
+        __syncthreads();
+        issue_b(kb + 2);                                     // its stage was read by kb - 2, retired in every warpgroup
+        wgmma_fence();
+        const int row = wg * 64 + kh * a.W + kw;
+        const uint64_t da = make_sw128_desc_rows(slab_hi, row), dal = make_sw128_desc_rows(slab_lo, row);
+        const uint64_t db = make_sw128_desc(b_ring_u32 + (uint32_t)(kb % SLAB_B_STAGES) * SLAB_B_STAGE);
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {
+            wgmma_f16<2 * SLAB_N>(dm, da + 2 * kk, db + 2 * kk);   // Ah.[Bh | Bl]
+            wgmma_f16<SLAB_N>(dl, dal + 2 * kk, db + 2 * kk);      // Al.Bh
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (++kw == a.KW) { kw = 0; ++kh; }
+    }
+    wgmma_wait<0>();
+    wgmma_fence_operand(dm);
+    wgmma_fence_operand(dl);
+    cp_async_wait<0>();
+
+    // ---- epilogue: slot s of accumulator row 16 w + l / 4 (+ 8), stored only when it is an output position ----
+    const int w = t >> 5, l = t & 31;
+    int64_t m_of[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int64_t sl = s0 + wg * 64 + 16 * w + (l >> 2) + 8 * h;
+        const int64_t img = sl / HW;
+        const int rem = (int)(sl - img * HW);
+        const int oh = rem / a.W, ow = rem - oh * a.W;
+        m_of[h] = (img < n_img && oh < a.OH && ow < a.OW) ? (img * a.OH + oh) * a.OW + ow : -1;
+    }
+#pragma unroll
+    for (int i = 0; i < SLAB_N / 8; ++i) {
+        const int nb = 8 * i + 2 * (l & 3);
+        const EpiCoef c = epi_coef(a, nb);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            if (m_of[h] < 0) continue;
+            const int q = 4 * i + 2 * h;
+            epi_store<ENG_F16>(a, c, m_of[h], nb, dm[q] + (dm[SLAB_N / 2 + q] + dl[q]), dm[q + 1] + (dm[SLAB_N / 2 + q + 1] + dl[q + 1]),
+                               inv_scale);
+        }
+    }
+}
+
+// Does the slab kernel take this engine-3 layer?  Un-padded, stride-1 'valid' convolution, 64 -> 64 channels, no
+// folded pooling, and the slab plus the weight ring fit in shared memory.
+bool slab_covers(const ConvArgs &a)
+{
+    return a.wt_f16 && !(a.flags & ISS_F_SIGMOID) && a.C == SLAB_C && a.N == SLAB_N && a.K == a.KH * a.KW * a.C && a.pool_h == 0 &&
+           a.SH == 1 && a.SW == 1 && a.PT == 0 && a.PL == 0 && a.OH == a.H - a.KH + 1 && a.OW == a.W - a.KW + 1 &&
+           slab_smem(slab_rows(a.KH, a.KW, a.W)) <= SLAB_MAX_SMEM;
+}
+
+template <int MODE>
+int launch_slab(const ConvArgs &a, cudaStream_t st)
+{
+    const int rows = slab_rows(a.KH, a.KW, a.W), smem = slab_smem(rows);
+    auto kern = conv_slab_kernel<MODE>;
+    ISS_CUDA_OK(iss_optin_smem(reinterpret_cast<const void *>(kern), smem));
+    const int64_t n_img = a.M / ((int64_t)a.OH * a.OW);
+    const int64_t slots = ((n_img - 1) * a.H + a.OH - 1) * (int64_t)a.W + a.OW;    // through the last output position
+    const int64_t tiles = (slots + SLAB_TS - 1) / SLAB_TS;
+    ISS_REQUIRE(tiles < (1ll << 31), ISS_ERR_INVALID, "conv_slab: batch too large");
+    const FirstFuse ff = a.first ? *a.first : FirstFuse{};
+    kern<<<(unsigned)tiles, SLAB_THREADS, smem, st>>>(a, ff, reinterpret_cast<const unsigned char *>(a.wt_f16), a.wt_f16_inv_scale, rows);
     ISS_CUDA_OK(cudaGetLastError());
     iss_count_launch();
     return ISS_OK;
@@ -341,7 +521,10 @@ template <int BN>
 int launch_f16(const ConvArgs &a, cudaStream_t st)
 {
     const float s = a.wt_f16_inv_scale;
-    if (a.first) return launch_wg<ENG_F16, BN, LD_FIRST>(a, a.wt_f16, s, st);
+    if (slab_covers(a)) {
+        if (a.first) return launch_slab<LD_FIRST>(a, st);
+        return a.in_packed ? launch_slab<LD_PACKED>(a, st) : launch_slab<LD_F32>(a, st);
+    }
     if (a.pool_h > 0) return launch_wg<ENG_F16, BN, LD_POOL>(a, a.wt_f16, s, st);
     if (a.in_packed) return launch_wg<ENG_F16, BN, LD_PACKED>(a, a.wt_f16, s, st);
     return launch_wg<ENG_F16, BN, LD_F32>(a, a.wt_f16, s, st);
@@ -383,9 +566,7 @@ bool iss_conv_f16_covers(const ConvArgs &a)
     if (!a.wt_f16 || (a.flags & ISS_F_SIGMOID)) return false;
     if (a.C % HBK != 0 || a.N % 64 != 0 || a.K != a.KH * a.KW * a.C) return false;
     if (a.pool_h > 0 && (a.first || !a.in_packed || a.pool_h / 2 != a.H || a.pool_w / 2 != a.W)) return false;   // 2x2 / stride-2 'valid' pooling only
-    if (a.first && (a.C != HBK || a.SH != 1 || a.SW != 1 || a.PT != 0 || a.PL != 0 || a.OH != a.H - a.KH + 1 || a.OW != a.W - a.KW + 1 ||
-                    (a.flags & ISS_F_RESIDUAL)))
-        return false;
+    if (a.first && (!slab_covers(a) || (a.flags & ISS_F_RESIDUAL))) return false;    // the fused first layer runs in the slab kernel
     return true;
 }
 

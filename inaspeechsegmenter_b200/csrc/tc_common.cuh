@@ -35,8 +35,26 @@ __device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr)
     return d;
 }
 
+// The same operand read as a window of 64 rows starting at row `row` (any row) of a SWIZZLE_128B tile at the
+// 1024-byte-aligned address `tile` (the slab kernel's row-shifted A operand).  The rows were stored with chunk j at
+// j ^ (row & 7), i.e. swizzled by the shared-memory address bits [7, 10).  wgmma applies the swizzle to the address
+// bits as well, so the start address alone selects the window and the matrix base offset (bits 49-51) stays 0; setting
+// it to (start >> 7) & 7, as the PTX ISA describes for unaligned starts, reads wrong rows on H100
+// (tests/test_slab_kernel_gpu.py).
+__device__ __forceinline__ uint64_t make_sw128_desc_rows(uint32_t tile, int row)
+{
+    return make_sw128_desc(tile + (uint32_t)row * 128u);
+}
+
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+// a compiler barrier on accumulator registers: no other instruction defining them is moved across it
+template <int N>
+__device__ __forceinline__ void wgmma_fence_operand(float (&d)[N])
+{
+#pragma unroll
+    for (int q = 0; q < N; ++q) asm volatile("" : "+f"(d[q])::"memory");
+}
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
