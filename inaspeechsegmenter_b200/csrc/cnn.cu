@@ -197,7 +197,7 @@ conv_first_direct_kernel(const FirstArgs a)
                 for (int q = 0; q < 4; ++q) {
                     float v = acc[p][q] + eb[q];
                     if (a.flags & ISS_F_AFFINE_PRE) v = fmaf(v, es1[q], et1[q]);
-                    if (a.flags & ISS_F_RELU) v = fmaxf(v, 0.f);
+                    if (a.flags & ISS_F_RELU) v = iss_relu(v);
                     if (a.flags & ISS_F_SIGMOID) v = 1.f / (1.f + expf(-v));
                     if (a.flags & ISS_F_AFFINE_POST) v = fmaf(v, es2[q], et2[q]);
                     y[q] = v;

@@ -156,7 +156,7 @@ conv_gemm_f32_kernel(const ConvArgs a)
             float x = acc[i][j] + eb[j];
             if (a.flags & ISS_F_AFFINE_PRE) x = fmaf(x, es1[j], et1[j]);
             if (a.flags & ISS_F_RESIDUAL) { const int n = n0 + tx * TN + j; if (n < a.N) x += __ldg(a.residual + mr * a.N + n); }
-            if (a.flags & ISS_F_RELU) x = fmaxf(x, 0.f);
+            if (a.flags & ISS_F_RELU) x = iss_relu(x);
             if (a.flags & ISS_F_SIGMOID) x = 1.f / (1.f + expf(-x));
             if (a.flags & ISS_F_AFFINE_POST) x = fmaf(x, es2[j], et2[j]);
             v[j] = x;
@@ -213,7 +213,7 @@ dense_small_n_kernel(const ConvArgs a)
             const int n = lane;
             if (a.flags & ISS_F_BIAS) xv += a.bias[n];
             if (a.flags & ISS_F_AFFINE_PRE) xv = fmaf(xv, a.pre_scale[n], a.pre_shift[n]);
-            if (a.flags & ISS_F_RELU) xv = fmaxf(xv, 0.f);
+            if (a.flags & ISS_F_RELU) xv = iss_relu(xv);
             if (a.flags & ISS_F_SIGMOID) xv = 1.f / (1.f + expf(-xv));
             if (a.flags & ISS_F_AFFINE_POST) xv = fmaf(xv, a.post_scale[n], a.post_shift[n]);
             a.out[m * a.N + n] = xv;

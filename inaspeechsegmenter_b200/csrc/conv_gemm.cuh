@@ -27,6 +27,16 @@ __device__ __forceinline__ float iss_unpack_split(uint32_t w)
     return __half2float(__ushort_as_half((unsigned short)(w & 0xFFFFu))) + __half2float(__ushort_as_half((unsigned short)(w >> 16)));
 }
 
+// ReLU with TensorFlow's NaN semantics: relu(NaN) = NaN.  fmaxf(NaN, 0) is 0, which would turn a non-finite activation
+// (e.g. an fp16-split word past the fp16 range, hi = inf, lo = -inf) into a finite, wrong value downstream.
+// max.NaN.f32 (sm_80+) is the same single instruction as fmaxf with NaN propagation; equal bits for every other input.
+__device__ __forceinline__ float iss_relu(float v)
+{
+    float r;
+    asm("max.NaN.f32 %0, %1, 0f00000000;" : "=f"(r) : "f"(v));
+    return r;
+}
+
 #define ISS_F_RESIDUAL 64     /* internal: + residual[m][n] after the pre-affine, before ReLU */
 
 // First layer folded into the operand fill of the convolution behind it (conv_gemm_tc.cu, LD_FIRST): the

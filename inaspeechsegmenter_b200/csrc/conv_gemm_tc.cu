@@ -125,7 +125,7 @@ __device__ __forceinline__ void epi_store(const ConvArgs &a, const EpiCoef &c, i
             if (pre) v = fmaf(v, c.es1[q], c.et1[q]);
         }
         if (resid) v += rv[q];
-        if (relu) v = fmaxf(v, 0.f);
+        if (relu) v = iss_relu(v);
         if (post) v = fmaf(v, c.es2[q], c.et2[q]);
         y[q] = v;
     }
@@ -406,7 +406,7 @@ conv_slab_kernel(const ConvArgs a, const FirstFuse ff, const unsigned char *__re
 #pragma unroll
                     for (int e = 0; e < 4; ++e) {
                         float x = fmaf(hv[e], al[e], bh[e]) + fmaf(lv[e], al[e], bl[e]);
-                        if (ff.flags & ISS_F_RELU) x = fmaxf(x, 0.f);
+                        if (ff.flags & ISS_F_RELU) x = iss_relu(x);
                         if (ff.flags & ISS_F_AFFINE_POST) {
                             const int c = j * 8 + 4 * q + e;
                             x = fmaf(x, __ldg(ff.post_scale + c), __ldg(ff.post_shift + c));

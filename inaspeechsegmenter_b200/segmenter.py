@@ -142,7 +142,17 @@ class DnnSegmenter:
         self.last_probs = probs
         seg_off = np.concatenate(([0], np.cumsum([b - a for a, b in ranges]))).astype(np.int64)
         trans = engine.diag_trans_exp(self.viterbi_arg, len(self.outlabels))
-        states = engine.viterbi_segments(self.ctx, probs, seg_off, trans).cpu().numpy()
+        states = engine.viterbi_segments(self.ctx, probs, seg_off, trans)
+        # Non-finite posteriors (rows of non-finite patches are already 0.5) mean the network left the range of its GEMM
+        # engine: the fp16-split engine carries activations as fp16 hi / lo pairs, |x| < 65504.  The flag is computed on
+        # the device and comes back with the states, in the copy that synchronises anyway.
+        flag = torch.isfinite(probs).all().to(torch.uint8).view(1)
+        states = torch.cat((states, flag)).cpu().numpy()
+        if not states[-1]:
+            raise _lib.IssError('%s: the CNN returned non-finite posteriors: an activation left the fp16 range of the '
+                                'default fp16-split GEMM engine; run with ISS_B200_GEMM=tc_ts (3xTF32, fp32 range)'
+                                % type(self).__name__)
+        states = states[:-1]
         k = 0
         for lab, a, b in lseg:
             if lab != self.inlabel:
