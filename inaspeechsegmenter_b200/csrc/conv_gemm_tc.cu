@@ -134,6 +134,35 @@ __device__ __forceinline__ void epi_store(const ConvArgs &a, const EpiCoef &c, i
     else *reinterpret_cast<float2 *>(dst) = make_float2(y[0], y[1]);
 }
 
+// The same epilogue for the single engine-3 output (m, n) (the slab kernel, whose accumulator rows are channels).
+struct EpiCoef1 {
+    float eb, es1, et1, es2, et2;
+};
+
+__device__ __forceinline__ EpiCoef1 epi_coef1(const ConvArgs &a, int n)
+{
+    const bool pre = a.flags & ISS_F_AFFINE_PRE, post = a.flags & ISS_F_AFFINE_POST;
+    EpiCoef1 c;
+    c.eb = (a.flags & ISS_F_BIAS) ? __ldg(a.bias + n) : 0.f;
+    c.es1 = pre ? __ldg(a.pre_scale + n) : 1.f;  c.et1 = pre ? __ldg(a.pre_shift + n) : 0.f;
+    c.es2 = post ? __ldg(a.post_scale + n) : 1.f; c.et2 = post ? __ldg(a.post_shift + n) : 0.f;
+    return c;
+}
+
+__device__ __forceinline__ void epi_store1(const ConvArgs &a, const EpiCoef1 &c, int64_t m, int n, float y, float inv_scale)
+{
+    float v = fmaf(y, inv_scale * c.es1, fmaf(c.eb, c.es1, c.et1));
+    if (a.flags & ISS_F_RESIDUAL) {
+        const uint32_t rw = __ldg(reinterpret_cast<const uint32_t *>(a.residual + m * a.N + n));
+        v += a.residual_packed ? iss_unpack_split(rw) : __uint_as_float(rw);
+    }
+    if (a.flags & ISS_F_RELU) v = iss_relu(v);
+    if (a.flags & ISS_F_AFFINE_POST) v = fmaf(v, c.es2, c.et2);
+    float *dst = a.out + m * a.N + n;
+    if (a.out_packed) *reinterpret_cast<uint32_t *>(dst) = iss_pack_split(v);
+    else *dst = v;
+}
+
 template <int ENG, int BN, int MODE>
 __global__ void __launch_bounds__(THREADS, 1)
 conv_gemm_wg_kernel(const ConvArgs a, const unsigned char *__restrict__ wt, float inv_scale)
@@ -335,183 +364,265 @@ int launch_wg(const ConvArgs &a, const void *wt, float inv_scale, cudaStream_t s
 
 // ============================ slab kernel: un-padded, stride-1 engine-3 convolutions with C = N = 64 ============================
 // The input of a batch is read as ONE tall image, pixel p = (img * H + ih) * W + iw, and every output slot gets the same
-// numbering, s = (img * H + oh) * W + ow.  The A operand of tap (kh, kw) for the slots s0 .. s0 + 63 is then the 64
-// consecutive pixels from s0 + kh * W + kw.  A CTA owns the slots s0 .. s0 + 255 (four warpgroups of 64); it evaluates,
-// splits and stores the pixels s0 .. s0 + 255 + (KH - 1) W + KW - 1 once into a SWIZZLE_128B hi plane and lo plane (the
-// "slab"), and every tap's A tile is a row-shifted window of it, addressed by the wgmma descriptor alone.  So each input
-// value is filled about 1.3 times instead of KH * KW times.  Slots with oh >= OH or ow >= OW (and slots past the batch)
-// are computed and not stored.  Slab rows past the last pixel of the batch are zero.
-// The weight stage of a tap is the engine-3 image [hi: 64 rows | lo: 64 rows] x 128 B, read as ONE 128-row B operand, so
-// Ah.[Bh | Bl] is one m64n128k16 (accumulator columns 0..63 = Ah.Bh, 64..127 = Ah.Bl) and Al.Bh one m64n64k16 into its
-// own accumulator: A is read twice per k16 step instead of three times.  (wgmma orders accumulator accesses only between
-// instructions of one shape, so the two shapes never share registers.)
-constexpr int SLAB_TS = 256, SLAB_THREADS = 512, SLAB_C = 64, SLAB_N = 64;
+// numbering, s = (img * H + oh) * W + ow.  The operand of tap (kh, kw) for the slots s0 .. s0 + 127 is then the 128
+// consecutive pixels from s0 + kh * W + kw.  A tile is the slots s0 .. s0 + 255; its pixels
+// s0 .. s0 + 255 + (KH - 1) W + KW - 1 are evaluated, split and stored once into a SWIZZLE_128B hi plane and lo plane
+// (the "slab"), and every tap's slot operand is a row-shifted window of it, addressed by the wgmma descriptor alone.  So
+// each input value is filled about 1.3 times instead of KH * KW times.  Slots with oh >= OH or ow >= OW (and slots past
+// the batch) are computed and not stored.  Slab rows past the last pixel of the batch are zero.
+// The slots are the N side of the products and the 64 output channels the M side: the weight stage of a tap is the
+// engine-3 image [hi: 64 rows | lo: 64 rows] x 128 B, whose halves are the A operands Bh^T and Bl^T, and a consumer's 128
+// slots are one N = 128 window.  So the three products hh = Bh^T.Ah, hl = Bl^T.Ah and lh = Bh^T.Al are three
+// m64n128k16 per k16 step, each reading 6 KB of shared memory for 64 tensor clocks (with the slots on the M side they
+// were an m64n128 Ah.[Bh | Bl] and an m64n64 Al.Bh per 64 slots, 10 KB for 96 clocks, and the n64 shape alone needs the
+// whole 128 B/clk of shared-memory bandwidth).  Each accumulator element still sums the same products of one slot and
+// one channel in the same order, and the epilogue adds hh + (hl + lh) as before.
+//
+// The kernel is persistent and warp-specialized: one CTA per SM takes tiles blockIdx.x, blockIdx.x + gridDim.x, ... (in
+// increasing order, so neighbouring CTAs share the first-layer map and input rows in L2).  Warpgroup 0 produces: its
+// warp 0 streams the weight stage of every tap with one bulk copy into a ring of `stages` stages, its warps 1..3 fill the
+// slab of the next tile into one of `nbuf` slab buffers.  Warpgroups 1 and 2 consume: consumer c owns the slots
+// s0 + 128 c .. s0 + 128 c + 127 and issues, per tap, the wgmmas above.  Full / empty mbarriers hand every weight stage
+// and every slab buffer from producer to consumers and back.  setmaxnreg moves registers from the producer (which holds
+// no accumulators) to the consumers (3 x 64 accumulator registers each).  With two slab buffers the fill of tile t + 1
+// runs while the consumers compute tile t; where two slabs do not fit (tall filters) one buffer is refilled once both
+// consumers have retired their last wgmma on it.
+constexpr int SLAB_TS = 256, SLAB_C = 64, SLAB_N = 64;
+constexpr int SLAB_THREADS = 384;                       // producer warpgroup + two consumer warpgroups
+constexpr int SLAB_FILL_THREADS = 96;                   // producer warps 1..3
+constexpr int SLAB_CONSUMER_ARRIVALS = 8;               // lane 0 of each consumer warp
+// the launch gives every thread 168 registers (384 threads, one CTA per SM): 128 x 56 + 256 x 224 = 384 x 168
+constexpr int SLAB_PRODUCER_REGS = 56, SLAB_CONSUMER_REGS = 224;
 constexpr int SLAB_B_STAGE = 2 * SLAB_N * 128;          // hi | lo, 64 rows x 128 B each
-constexpr int SLAB_B_STAGES = 4;
+constexpr int SLAB_MAX_STAGES = 4, SLAB_MAX_BUF = 2;
+constexpr int SLAB_BAR_BYTES = 8 * 2 * (SLAB_MAX_STAGES + SLAB_MAX_BUF);
 constexpr int SLAB_MAX_SMEM = 227 * 1024;
 
-// slab rows of a tile (a multiple of 8, so that the lo plane stays 1024-byte aligned) and the kernel's shared memory
+// slab rows of a tile (a multiple of 8, so that the lo plane stays 1024-byte aligned) and the kernel's shared memory:
+// `stages` weight stages, `nbuf` slabs and 1024 bytes of alignment slack, which also hold the mbarriers
 int slab_rows(int KH, int KW, int W) { return (SLAB_TS + (KH - 1) * W + KW - 1 + 7) & ~7; }
-int slab_smem(int rows) { return SLAB_B_STAGES * SLAB_B_STAGE + 2 * rows * 128 + 1024; }
+int slab_smem(int rows, int nbuf, int stages) { return stages * SLAB_B_STAGE + nbuf * 2 * rows * 128 + 1024; }
+
+// one 16-byte chunk of the slab: chunk j of pixel row r (pixel s0 + r) at chunk j ^ (r & 7) of both planes
+template <int MODE>
+__device__ __forceinline__ void slab_fill_chunk(const ConvArgs &a, const FirstFuse &ff, uint32_t slab_hi, uint32_t slab_lo,
+                                                int64_t s0, int u, int64_t HW, int64_t npix)
+{
+    const int r = u >> 3, j = u & 7;
+    const int64_t p = s0 + r;
+    uint32_t hw[4] = {0u, 0u, 0u, 0u}, lw[4] = {0u, 0u, 0u, 0u};
+    if (p < npix) {
+        if constexpr (MODE == LD_FIRST) {                     // the first layer at pixel p, from the map Y of its own patch
+            const int64_t img = p / HW;
+            const int rem = (int)(p - img * HW);
+            const int ih = rem / a.W, iw = rem - ih * a.W;
+            const int64_t o = (((int64_t)__ldg(ff.row0 + img) - ff.y_f0 + ih) * a.W + iw) * SLAB_C + j * 8;
+            const float4 *yh = reinterpret_cast<const float4 *>(ff.Yh + o), *yl = reinterpret_cast<const float4 *>(ff.Yl + o);
+            const float4 *cf = reinterpret_cast<const float4 *>(ff.coef + img * (3 * SLAB_C) + j * 8);
+            float v[8];
+#pragma unroll
+            for (int q = 0; q < 2; ++q) {
+                const float4 h4 = __ldg(yh + q), l4 = __ldg(yl + q);
+                const float4 va = __ldg(cf + q), vh = __ldg(cf + SLAB_C / 4 + q), vl = __ldg(cf + 2 * (SLAB_C / 4) + q);
+                const float hv[4] = {h4.x, h4.y, h4.z, h4.w}, lv[4] = {l4.x, l4.y, l4.z, l4.w};
+                const float al[4] = {va.x, va.y, va.z, va.w}, bh[4] = {vh.x, vh.y, vh.z, vh.w}, bl[4] = {vl.x, vl.y, vl.z, vl.w};
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    float x = fmaf(hv[e], al[e], bh[e]) + fmaf(lv[e], al[e], bl[e]);
+                    if (ff.flags & ISS_F_RELU) x = iss_relu(x);
+                    if (ff.flags & ISS_F_AFFINE_POST) {
+                        const int c = j * 8 + 4 * q + e;
+                        x = fmaf(x, __ldg(ff.post_scale + c), __ldg(ff.post_shift + c));
+                    }
+                    v[4 * q + e] = x;
+                }
+            }
+            split_f16(v, hw, lw);
+        } else {                                              // NHWC pixel p of the batch is the tall image's pixel p
+            const uint4 *src = reinterpret_cast<const uint4 *>(a.in + p * SLAB_C + j * 8);
+            const uint4 u0 = __ldg(src), u1 = __ldg(src + 1);
+            if constexpr (MODE == LD_PACKED) {
+                const uint32_t w[8] = {u0.x, u0.y, u0.z, u0.w, u1.x, u1.y, u1.z, u1.w};
+                words_to_planes(w, hw, lw);
+            } else {
+                static_assert(MODE == LD_F32, "slab fill modes: LD_F32, LD_PACKED, LD_FIRST");
+                const float v[8] = {__uint_as_float(u0.x), __uint_as_float(u0.y), __uint_as_float(u0.z), __uint_as_float(u0.w),
+                                    __uint_as_float(u1.x), __uint_as_float(u1.y), __uint_as_float(u1.z), __uint_as_float(u1.w)};
+                split_f16(v, hw, lw);
+            }
+        }
+    }
+    const uint32_t dst = (uint32_t)r * 128u + ((uint32_t)(j ^ (r & 7)) << 4);
+    sts128(slab_hi + dst, hw[0], hw[1], hw[2], hw[3]);
+    sts128(slab_lo + dst, lw[0], lw[1], lw[2], lw[3]);
+}
 
 template <int MODE>
 __global__ void __launch_bounds__(SLAB_THREADS, 1)
-conv_slab_kernel(const ConvArgs a, const FirstFuse ff, const unsigned char *__restrict__ wt, float inv_scale, int rows)
+conv_slab_kernel(const ConvArgs a, const FirstFuse ff, const unsigned char *__restrict__ wt, float inv_scale, int rows,
+                 int64_t tiles, int nbuf, int stages)
 {
     extern __shared__ unsigned char smem_dyn[];
-    unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
-    const uint32_t b_ring_u32 = smem_u32(smem);
-    const uint32_t slab_hi = b_ring_u32 + SLAB_B_STAGES * SLAB_B_STAGE, slab_lo = slab_hi + (uint32_t)rows * 128u;
+    const uint32_t base = smem_u32(smem_dyn);
+    const uint32_t ring = (base + 1023u) & ~1023u;           // weight stages, then the slabs: 1024-byte aligned
+    const uint32_t slab0 = ring + (uint32_t)stages * SLAB_B_STAGE, slab_bytes = (uint32_t)rows * 256u;
+    // the mbarriers go into the bytes the alignment skips when they fit there, else right after the slabs: either way
+    // inside the 1024 bytes of slack that slab_smem counts
+    const uint32_t bars = ring - base >= (uint32_t)SLAB_BAR_BYTES ? base : slab0 + (uint32_t)nbuf * slab_bytes;
+    const uint32_t wfull = bars, wempty = bars + 8 * SLAB_MAX_STAGES;                   // + 8 * stage
+    const uint32_t sfull = bars + 16 * SLAB_MAX_STAGES, sempty = sfull + 8 * SLAB_MAX_BUF;  // + 8 * buffer
 
-    const int tid = threadIdx.x, wg = tid >> 7, t = tid & 127;
-    const int64_t s0 = (int64_t)blockIdx.x * SLAB_TS;
+    const int tid = threadIdx.x, wg = tid >> 7;
+    if (tid == 0) {
+        for (int s = 0; s < stages; ++s) { mbar_init(wfull + 8 * s, 1); mbar_init(wempty + 8 * s, SLAB_CONSUMER_ARRIVALS); }
+        for (int b = 0; b < nbuf; ++b) { mbar_init(sfull + 8 * b, SLAB_FILL_THREADS); mbar_init(sempty + 8 * b, SLAB_CONSUMER_ARRIVALS); }
+        fence_mbar_init();
+    }
+    __syncthreads();
+
     const int nkb = a.KH * a.KW;                             // one k-block (64 channels) per tap
     const int64_t HW = (int64_t)a.H * a.W;
     const int64_t n_img = a.M / ((int64_t)a.OH * a.OW);
     const int64_t npix = n_img * HW;
 
-    auto issue_b = [&](int kb) {
-        if (kb < nkb) {
-            const unsigned char *src = wt + (size_t)kb * SLAB_B_STAGE;
-            const uint32_t dst = b_ring_u32 + (uint32_t)(kb % SLAB_B_STAGES) * SLAB_B_STAGE;
-#pragma unroll
-            for (int o = tid * 16; o < SLAB_B_STAGE; o += SLAB_THREADS * 16) cp_async16_u32(dst + o, src + o, 16);
-        }
-        cp_async_commit();                                   // (empty groups keep the group count uniform)
-    };
-    issue_b(0);
-    issue_b(1);
-
-    // ---- the slab: 16-byte chunk j of pixel row r at chunk j ^ (r & 7) of both planes ----
-#pragma unroll 2
-    for (int u = tid; u < rows * 8; u += SLAB_THREADS) {
-        const int r = u >> 3, j = u & 7;
-        const int64_t p = s0 + r;
-        uint32_t hw[4] = {0u, 0u, 0u, 0u}, lw[4] = {0u, 0u, 0u, 0u};
-        if (p < npix) {
-            if constexpr (MODE == LD_FIRST) {                 // the first layer at pixel p, from the map Y of its own patch
-                const int64_t img = p / HW;
-                const int rem = (int)(p - img * HW);
-                const int ih = rem / a.W, iw = rem - ih * a.W;
-                const int64_t o = (((int64_t)__ldg(ff.row0 + img) - ff.y_f0 + ih) * a.W + iw) * SLAB_C + j * 8;
-                const float4 *yh = reinterpret_cast<const float4 *>(ff.Yh + o), *yl = reinterpret_cast<const float4 *>(ff.Yl + o);
-                const float4 *cf = reinterpret_cast<const float4 *>(ff.coef + img * (3 * SLAB_C) + j * 8);
-                float v[8];
-#pragma unroll
-                for (int q = 0; q < 2; ++q) {
-                    const float4 h4 = __ldg(yh + q), l4 = __ldg(yl + q);
-                    const float4 va = __ldg(cf + q), vh = __ldg(cf + SLAB_C / 4 + q), vl = __ldg(cf + 2 * (SLAB_C / 4) + q);
-                    const float hv[4] = {h4.x, h4.y, h4.z, h4.w}, lv[4] = {l4.x, l4.y, l4.z, l4.w};
-                    const float al[4] = {va.x, va.y, va.z, va.w}, bh[4] = {vh.x, vh.y, vh.z, vh.w}, bl[4] = {vl.x, vl.y, vl.z, vl.w};
-#pragma unroll
-                    for (int e = 0; e < 4; ++e) {
-                        float x = fmaf(hv[e], al[e], bh[e]) + fmaf(lv[e], al[e], bl[e]);
-                        if (ff.flags & ISS_F_RELU) x = iss_relu(x);
-                        if (ff.flags & ISS_F_AFFINE_POST) {
-                            const int c = j * 8 + 4 * q + e;
-                            x = fmaf(x, __ldg(ff.post_scale + c), __ldg(ff.post_shift + c));
-                        }
-                        v[4 * q + e] = x;
+    if (wg == 0) {
+        // ============================ producer ============================
+        setmaxnreg_dec<SLAB_PRODUCER_REGS>();
+        if (tid < 32) {                                      // warp 0: the weight stages of every tap of every tile
+            if (tid == 0) {
+                int s = 0;
+                uint32_t ph = 0;
+                for (int64_t tile = blockIdx.x; tile < tiles; tile += gridDim.x)
+                    for (int kb = 0; kb < nkb; ++kb) {
+                        mbar_wait(wempty + 8 * s, ph ^ 1);   // both consumers retired the wgmmas that read the stage
+                        mbar_arrive_expect_tx(wfull + 8 * s, SLAB_B_STAGE);
+                        bulk_copy_g2s(ring + (uint32_t)s * SLAB_B_STAGE, wt + (size_t)kb * SLAB_B_STAGE, SLAB_B_STAGE, wfull + 8 * s);
+                        if (++s == stages) { s = 0; ph ^= 1; }
                     }
-                }
-                split_f16(v, hw, lw);
-            } else {                                          // NHWC pixel p of the batch is the tall image's pixel p
-                const uint4 *src = reinterpret_cast<const uint4 *>(a.in + p * SLAB_C + j * 8);
-                const uint4 u0 = __ldg(src), u1 = __ldg(src + 1);
-                if constexpr (MODE == LD_PACKED) {
-                    const uint32_t w[8] = {u0.x, u0.y, u0.z, u0.w, u1.x, u1.y, u1.z, u1.w};
-                    words_to_planes(w, hw, lw);
-                } else {
-                    static_assert(MODE == LD_F32, "slab fill modes: LD_F32, LD_PACKED, LD_FIRST");
-                    const float v[8] = {__uint_as_float(u0.x), __uint_as_float(u0.y), __uint_as_float(u0.z), __uint_as_float(u0.w),
-                                        __uint_as_float(u1.x), __uint_as_float(u1.y), __uint_as_float(u1.z), __uint_as_float(u1.w)};
-                    split_f16(v, hw, lw);
-                }
+            }
+        } else {                                             // warps 1..3: the slab of every tile
+            int b = 0;
+            uint32_t ph = 0;
+            for (int64_t tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+                mbar_wait(sempty + 8 * b, ph ^ 1);           // both consumers retired their last wgmma on this buffer
+                const uint32_t hi = slab0 + (uint32_t)b * slab_bytes, lo = hi + (uint32_t)rows * 128u;
+#pragma unroll 1
+                for (int u = tid - 32; u < rows * 8; u += SLAB_FILL_THREADS)
+                    slab_fill_chunk<MODE>(a, ff, hi, lo, tile * SLAB_TS, u, HW, npix);
+                fence_proxy_async();                         // this thread's slab stores, visible to wgmma
+                mbar_arrive(sfull + 8 * b);
+                if (++b == nbuf) { b = 0; ph ^= 1; }
             }
         }
-        const uint32_t dst = (uint32_t)r * 128u + ((uint32_t)(j ^ (r & 7)) << 4);
-        sts128(slab_hi + dst, hw[0], hw[1], hw[2], hw[3]);
-        sts128(slab_lo + dst, lw[0], lw[1], lw[2], lw[3]);
+        return;
     }
 
-    float dm[SLAB_N], dl[SLAB_N / 2];                        // dm: [Ah.Bh | Ah.Bl] (n128), dl: Al.Bh (n64)
+    // ============================ consumers ============================
+    setmaxnreg_inc<SLAB_CONSUMER_REGS>();
+    const int c = wg - 1, t = tid & 127, w = t >> 5, l = t & 31;
+    int s = 0, b = 0;
+    uint32_t wph = 0, sph = 0;
+    for (int64_t tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+        const int64_t s0 = tile * SLAB_TS;
+        // the consumer's 128 slots as the N side of three m64n128 products, output channels as the M side:
+        // hh = Bh^T.Ah, hl = Bl^T.Ah, lh = Bh^T.Al (accumulator row = channel, column = slot)
+        float hh[SLAB_N], hl[SLAB_N], lh[SLAB_N];
 #pragma unroll
-    for (int q = 0; q < SLAB_N; ++q) dm[q] = 0.f;
-#pragma unroll
-    for (int q = 0; q < SLAB_N / 2; ++q) dl[q] = 0.f;
-    wgmma_fence_operand(dm);                                 // keep the zeroing out of the wgmma pipeline (ptxas would
-    wgmma_fence_operand(dl);                                 // otherwise serialize every wgmma of the loop)
+        for (int q = 0; q < SLAB_N; ++q) { hh[q] = 0.f; hl[q] = 0.f; lh[q] = 0.f; }
+        wgmma_fence_operand(hh);                             // keep the zeroing out of the wgmma pipeline (ptxas would
+        wgmma_fence_operand(hl);                             // otherwise serialize every wgmma of the loop)
+        wgmma_fence_operand(lh);
+        mbar_wait(sfull + 8 * b, sph);
+        const uint32_t slab_hi = slab0 + (uint32_t)b * slab_bytes, slab_lo = slab_hi + (uint32_t)rows * 128u;
 
-    int kh = 0, kw = 0;
-    for (int kb = 0; kb < nkb; ++kb) {
-        cp_async_wait<1>();                                  // weights of kb landed (kb + 1 may still be in flight)
-        fence_proxy_async();                                 // (and, at kb = 0, this thread's slab stores)
-        __syncthreads();
-        issue_b(kb + 2);                                     // its stage was read by kb - 2, retired in every warpgroup
-        wgmma_fence();
-        const int row = wg * 64 + kh * a.W + kw;
-        const uint64_t da = make_sw128_desc_rows(slab_hi, row), dal = make_sw128_desc_rows(slab_lo, row);
-        const uint64_t db = make_sw128_desc(b_ring_u32 + (uint32_t)(kb % SLAB_B_STAGES) * SLAB_B_STAGE);
+        int kh = 0, kw = 0, prev = -1;
+        for (int kb = 0; kb < nkb; ++kb) {
+            mbar_wait(wfull + 8 * s, wph);                   // the weights of this tap landed
+            wgmma_fence();
+            const uint32_t stage = ring + (uint32_t)s * SLAB_B_STAGE;
+            const uint64_t dwh = make_sw128_desc(stage), dwl = make_sw128_desc(stage + SLAB_N * 128);
+            const int row = 128 * c + kh * a.W + kw;
+            const uint64_t dxh = make_sw128_desc_rows(slab_hi, row), dxl = make_sw128_desc_rows(slab_lo, row);
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {
-            wgmma_f16<2 * SLAB_N>(dm, da + 2 * kk, db + 2 * kk);   // Ah.[Bh | Bl]
-            wgmma_f16<SLAB_N>(dl, dal + 2 * kk, db + 2 * kk);      // Al.Bh
+            for (int kk = 0; kk < 4; ++kk) {
+                wgmma_f16<2 * SLAB_N>(hh, dwh + 2 * kk, dxh + 2 * kk);
+                wgmma_f16<2 * SLAB_N>(hl, dwl + 2 * kk, dxh + 2 * kk);
+                wgmma_f16<2 * SLAB_N>(lh, dwh + 2 * kk, dxl + 2 * kk);
+            }
+            wgmma_commit();
+            wgmma_wait<1>();                                 // the previous tap's wgmmas retired: release its stage
+            if (prev >= 0 && l == 0) mbar_arrive(wempty + 8 * prev);
+            prev = s;
+            if (++s == stages) { s = 0; wph ^= 1; }
+            if (++kw == a.KW) { kw = 0; ++kh; }
         }
-        wgmma_commit();
-        wgmma_wait<1>();
-        if (++kw == a.KW) { kw = 0; ++kh; }
-    }
-    wgmma_wait<0>();
-    wgmma_fence_operand(dm);
-    wgmma_fence_operand(dl);
-    cp_async_wait<0>();
+        wgmma_wait<0>();
+        wgmma_fence_operand(hh);
+        wgmma_fence_operand(hl);
+        wgmma_fence_operand(lh);
+        if (l == 0) { mbar_arrive(wempty + 8 * prev); mbar_arrive(sempty + 8 * b); }
+        if (++b == nbuf) { b = 0; sph ^= 1; }
 
-    // ---- epilogue: slot s of accumulator row 16 w + l / 4 (+ 8), stored only when it is an output position ----
-    const int w = t >> 5, l = t & 31;
-    int64_t m_of[2];
+        // ---- epilogue: register q = 4 i + 2 h + e holds channel 16 w + l / 4 + 8 h of slot
+        //      s0 + 128 c + 8 i + 2 (l % 4) + e, stored only when the slot is an output position ----
+        EpiCoef1 cf[2];
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-        const int64_t sl = s0 + wg * 64 + 16 * w + (l >> 2) + 8 * h;
-        const int64_t img = sl / HW;
-        const int rem = (int)(sl - img * HW);
-        const int oh = rem / a.W, ow = rem - oh * a.W;
-        m_of[h] = (img < n_img && oh < a.OH && ow < a.OW) ? (img * a.OH + oh) * a.OW + ow : -1;
-    }
+        for (int h = 0; h < 2; ++h) cf[h] = epi_coef1(a, 16 * w + (l >> 2) + 8 * h);
+        const int64_t sl0 = s0 + 128 * c + 2 * (l & 3);
+        int64_t img = sl0 / HW;                              // (img, oh, ow) of slot sl0 + 8 i, advanced with i
+        int rem = (int)(sl0 - img * HW);
+        int oh = rem / a.W, ow = rem - oh * a.W;
 #pragma unroll
-    for (int i = 0; i < SLAB_N / 8; ++i) {
-        const int nb = 8 * i + 2 * (l & 3);
-        const EpiCoef c = epi_coef(a, nb);
+        for (int i = 0; i < 2 * SLAB_N / 8; ++i) {
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            if (m_of[h] < 0) continue;
-            const int q = 4 * i + 2 * h;
-            epi_store<ENG_F16>(a, c, m_of[h], nb, dm[q] + (dm[SLAB_N / 2 + q] + dl[q]), dm[q + 1] + (dm[SLAB_N / 2 + q + 1] + dl[q + 1]),
-                               inv_scale);
+            for (int e = 0; e < 2; ++e) {
+                int64_t ie = img;
+                int he = oh, we = ow + e;
+                if (we == a.W) { we = 0; if (++he == a.H) { he = 0; ++ie; } }
+                if (ie < n_img && he < a.OH && we < a.OW) {
+                    const int64_t m = (ie * a.OH + he) * a.OW + we;
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const int q = 4 * i + 2 * h + e;
+                        epi_store1(a, cf[h], m, 16 * w + (l >> 2) + 8 * h, hh[q] + (hl[q] + lh[q]), inv_scale);
+                    }
+                }
+            }
+            ow += 8;
+            while (ow >= a.W) { ow -= a.W; if (++oh == a.H) { oh = 0; ++img; } }
         }
     }
 }
 
 // Does the slab kernel take this engine-3 layer?  Un-padded, stride-1 'valid' convolution, 64 -> 64 channels, no
-// folded pooling, and the slab plus the weight ring fit in shared memory.
+// folded pooling, and one slab plus a four-stage weight ring fit in shared memory.
 bool slab_covers(const ConvArgs &a)
 {
     return a.wt_f16 && !(a.flags & ISS_F_SIGMOID) && a.C == SLAB_C && a.N == SLAB_N && a.K == a.KH * a.KW * a.C && a.pool_h == 0 &&
            a.SH == 1 && a.SW == 1 && a.PT == 0 && a.PL == 0 && a.OH == a.H - a.KH + 1 && a.OW == a.W - a.KW + 1 &&
-           slab_smem(slab_rows(a.KH, a.KW, a.W)) <= SLAB_MAX_SMEM;
+           slab_smem(slab_rows(a.KH, a.KW, a.W), 1, SLAB_MAX_STAGES) <= SLAB_MAX_SMEM;
 }
 
 template <int MODE>
 int launch_slab(const ConvArgs &a, cudaStream_t st)
 {
-    const int rows = slab_rows(a.KH, a.KW, a.W), smem = slab_smem(rows);
+    const int rows = slab_rows(a.KH, a.KW, a.W);
+    // two slabs (the fill of the next tile overlaps the current one) and a three-stage ring where they fit, else one
+    // slab and four stages
+    const bool pingpong = slab_smem(rows, 2, 3) <= SLAB_MAX_SMEM;
+    const int nbuf = pingpong ? 2 : 1, stages = pingpong ? 3 : SLAB_MAX_STAGES, smem = slab_smem(rows, nbuf, stages);
     auto kern = conv_slab_kernel<MODE>;
     ISS_CUDA_OK(iss_optin_smem(reinterpret_cast<const void *>(kern), smem));
     const int64_t n_img = a.M / ((int64_t)a.OH * a.OW);
     const int64_t slots = ((n_img - 1) * a.H + a.OH - 1) * (int64_t)a.W + a.OW;    // through the last output position
     const int64_t tiles = (slots + SLAB_TS - 1) / SLAB_TS;
-    ISS_REQUIRE(tiles < (1ll << 31), ISS_ERR_INVALID, "conv_slab: batch too large");
+    int dev = 0, sms = 0;
+    ISS_CUDA_OK(cudaGetDevice(&dev));
+    ISS_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    const unsigned grid = (unsigned)(tiles < sms ? tiles : sms);
     const FirstFuse ff = a.first ? *a.first : FirstFuse{};
-    kern<<<(unsigned)tiles, SLAB_THREADS, smem, st>>>(a, ff, reinterpret_cast<const unsigned char *>(a.wt_f16), a.wt_f16_inv_scale, rows);
+    kern<<<grid, SLAB_THREADS, smem, st>>>(a, ff, reinterpret_cast<const unsigned char *>(a.wt_f16), a.wt_f16_inv_scale, rows,
+                                           tiles, nbuf, stages);
     ISS_CUDA_OK(cudaGetLastError());
     iss_count_launch();
     return ISS_OK;

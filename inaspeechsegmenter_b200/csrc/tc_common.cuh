@@ -1,5 +1,6 @@
-// tc_common.cuh -- PTX wrappers of the Hopper (sm_90a) tensor-core GEMM kernel (conv_gemm_tc.cu): cp.async, the
-// shared-memory matrix descriptor of wgmma, and wgmma.mma_async for the shapes that kernel issues.
+// tc_common.cuh -- PTX wrappers of the Hopper (sm_90a) tensor-core GEMM kernels (conv_gemm_tc.cu): cp.async, bulk
+// copies and mbarriers, setmaxnreg, the shared-memory matrix descriptor of wgmma, and wgmma.mma_async for the shapes
+// those kernels issue.
 #pragma once
 #include "conv_gemm.cuh"
 
@@ -17,6 +18,39 @@ __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_gr
 
 // generic-proxy shared-memory writes (st.shared, cp.async) made visible to the async proxy that wgmma reads through
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+// mbarriers (shared::cta addresses).  A wait on parity ph returns once the phase of that parity has completed; on a
+// fresh barrier a wait on parity 1 returns at once, which is how a producer's first pass over an "empty" barrier goes.
+__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count)
+{
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
+}
+// makes the initialisations visible to the async proxy (cp.async.bulk completes on these barriers)
+__device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+__device__ __forceinline__ void mbar_arrive(uint32_t bar)
+{
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes)
+{
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity)
+{
+    asm volatile("{\n\t.reg .pred p;\n\tWAIT:\n\t"
+                 "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
+                 "@!p bra WAIT;\n\t}" ::"r"(bar), "r"(parity) : "memory");
+}
+// one bulk copy global -> shared (16-byte aligned, size a multiple of 16) that completes `bytes` of transaction on bar
+__device__ __forceinline__ void bulk_copy_g2s(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar)
+{
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
+}
+
+// per-thread register budget of the executing warpgroup (all its warps execute it); the CTA's pool is fixed at launch
+template <int R> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
 __device__ __forceinline__ void sts128(uint32_t addr, uint32_t x, uint32_t y, uint32_t z, uint32_t w)
 {
