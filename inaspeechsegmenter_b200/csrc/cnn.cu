@@ -39,10 +39,7 @@ struct Layer {
     iss_layer_desc d;
     int in_h, in_w, in_c;
     int out_h, out_w, out_c;
-    float *d_wt = nullptr;      // tensor-core weights [2][N][Kp] (eligible layers only)
-    int Kp = 0;
-    void *d_wt_f16 = nullptr;   // fp16 hi/lo image of engine 3 (KHxKW > 1 convolutions with K % 64 == 0, N % 64 == 0)
-    float f16_inv_scale = 1.f;
+    TcWeights wt;
 };
 
 }  // namespace
@@ -456,14 +453,8 @@ extern "C" int iss_cnn_create(iss_ctx *ctx, const iss_layer_desc *layers, int n_
         const iss_layer_desc &d = L.d;
         if (d.kind == ISS_LAYER_MAXPOOL) continue;
         const int K = (d.kind == ISS_LAYER_DENSE) ? d.cin : d.kh * d.kw * d.cin;
-        const int C = (d.kind == ISS_LAYER_DENSE) ? d.cin : d.cin;
-        if (C % 32 != 0 || K % 32 != 0 || d.cout % 32 != 0) continue;
-        int rc = iss_prepare_tc_weights(h_blob + d.w_off, K, d.cout, &L.d_wt, &L.Kp);
+        const int rc = iss_prepare_weights(h_blob + d.w_off, d.cin, K, d.cout, true, &L.wt);
         if (rc != ISS_OK) { iss_cnn_destroy(m); return rc; }
-        if (d.cin % 64 == 0) {                                    // fp16-split engine (engine 3)
-            rc = iss_prepare_f16_weights(h_blob + d.w_off, K, d.cout, &L.d_wt_f16, &L.f16_inv_scale);
-            if (rc != ISS_OK) { iss_cnn_destroy(m); return rc; }
-        }
     }
     {   // S_c = sum of the first layer's taps (float64), for the fused first layer
         const iss_layer_desc &d0 = m->layers[0].d;
@@ -485,7 +476,7 @@ extern "C" int iss_cnn_destroy(iss_cnn *cnn)
     if (!cnn) return ISS_OK;
     cudaSetDevice(cnn->ctx->device);
     for (cudaEvent_t ev : cnn->prof_ev) cudaEventDestroy(ev);
-    for (Layer &L : cnn->layers) { if (L.d_wt) cudaFree(L.d_wt); if (L.d_wt_f16) cudaFree(L.d_wt_f16); }
+    for (Layer &L : cnn->layers) iss_free_weights(&L.wt);
     if (cnn->d_blob) cudaFree(cnn->d_blob);
     if (cnn->d_first_S) cudaFree(cnn->d_first_S);
     delete cnn;
@@ -524,45 +515,116 @@ extern "C" int64_t iss_cnn_workspace_bytes(const iss_cnn *cnn, int64_t n, int n_
 
 namespace {
 
-// geometry + weight pointers of a Conv2D / Dense layer for `nb` patches (the fields iss_launch_conv dispatches on)
-void fill_conv_args(const Layer &Lr, int64_t nb, ConvArgs &a)
-{
-    const iss_layer_desc &d = Lr.d;
-    if (Lr.d_wt) { a.wt_hi = Lr.d_wt; a.wt_lo = Lr.d_wt + (size_t)d.cout * Lr.Kp; a.wt_tiled = Lr.d_wt + 2 * (size_t)d.cout * Lr.Kp; a.Kp = Lr.Kp; }
-    a.wt_f16 = Lr.d_wt_f16; a.wt_f16_inv_scale = Lr.f16_inv_scale;
-    a.N = d.cout;
-    if (d.kind == ISS_LAYER_DENSE) {
-        a.M = nb; a.K = d.cin; a.H = 1; a.W = 1; a.C = d.cin; a.OH = 1; a.OW = 1;
-        a.KH = 1; a.KW = 1; a.SH = 1; a.SW = 1; a.PT = 0; a.PL = 0;
-    } else {
-        a.M = nb * Lr.out_h * Lr.out_w; a.K = d.kh * d.kw * d.cin;
-        a.H = Lr.in_h; a.W = Lr.in_w; a.C = Lr.in_c; a.OH = Lr.out_h; a.OW = Lr.out_w;
-        a.KH = d.kh; a.KW = d.kw; a.SH = d.sh; a.SW = d.sw; a.PT = d.pad_top; a.PL = d.pad_left;
-    }
-}
+// How iss_cnn_forward runs a layer
+enum class Step {
+    FOLDED_POOL,        // 2x2 / stride-2 pooling taken in the next convolution's operand fill: nothing runs
+    POOL, POOL_VEC4, POOL_PACKED,   // maxpool_nhwc_kernel, maxpool_nhwc_vec4_kernel, maxpool_nhwc_packed_kernel
+    FIRST_DIRECT,       // conv_first_direct_kernel (unless the batch folds layer 0 into layer 1)
+    FIRST_GENERIC,      // the fp32 implicit GEMM gathering from the log-mel rows
+    CONV,               // iss_launch_conv
+};
 
-// Will this Conv2D / Dense layer run on the fp16-split engine?  Only that engine reads / writes split-half words.
-// ('same' padding with an extra bottom / right row is covered: rows past the input are zero-filled.)
-bool f16_engine_covers(const Layer &L, const ConvArgs &a)
-{
-    return L.d.kind != ISS_LAYER_MAXPOOL && iss_conv_f16_covers(a);
-}
+struct LayerPlan {
+    Step step;
+    // every step but the pooling ones: all but in, out, M, `first` and the patch arrays of the batch.  in_packed /
+    // out_packed are the activation formats, pool_h / pool_w the dims of a pooling folded into this layer.
+    ConvArgs a;
+};
 
-// Should the tensor produced by layer `li` be stored as split-half words?  Yes iff the next compute layer
-// (pooling layers in between keep the format) is a convolution the fp16-split engine takes.
-bool wants_packed_output(const iss_cnn *cnn, size_t li, int64_t nb)
+// The kernel and activation formats of every layer for one call of iss_cnn_forward, from the GEMM mode, the switches
+// ISS_B200_FUSE_POOL / ISS_B200_FUSE_FIRST ("0": pooling / first layer as their own kernels) and the profiled layer,
+// all of which may change between calls.  *fuse_first: layer 0 may be folded into layer 1 (first_map: the workspace
+// holds the fused first layer's map and the ranges ascend), decided per batch by the frames its patches span.
+int plan_forward(const iss_cnn *cnn, int mode, bool first_map, std::vector<LayerPlan> &plan, bool *fuse_first)
 {
-    if (iss_get_gemm_mode() != ISS_GEMM_TC_F16) return false;
-    size_t j = li + 1;
-    while (j < cnn->layers.size() && cnn->layers[j].d.kind == ISS_LAYER_MAXPOOL) {
-        if (cnn->layers[j].in_c % 4 != 0) return false;          // the packed pooling kernel moves 4 channels per thread
-        ++j;
+    const char *e = getenv("ISS_B200_FUSE_POOL");
+    const bool fuse_pool = !(e && e[0] == '0');
+    e = getenv("ISS_B200_FUSE_FIRST");
+    const bool fuse_first_on = !(e && e[0] == '0');
+    const size_t n = cnn->layers.size();
+    plan.assign(n, LayerPlan{});
+    for (size_t li = 0; li < n; ++li) {
+        const Layer &Lr = cnn->layers[li];
+        const iss_layer_desc &d = Lr.d;
+        if (d.kind == ISS_LAYER_MAXPOOL) continue;
+        const float *blob = cnn->d_blob;
+        ConvArgs &a = plan[li].a;
+        a.w = blob + d.w_off;
+        a.bias = (d.flags & ISS_F_BIAS) ? blob + d.bias_off : nullptr;
+        a.pre_scale = (d.flags & ISS_F_AFFINE_PRE) ? blob + d.pre_scale_off : nullptr;
+        a.pre_shift = (d.flags & ISS_F_AFFINE_PRE) ? blob + d.pre_shift_off : nullptr;
+        a.post_scale = (d.flags & ISS_F_AFFINE_POST) ? blob + d.post_scale_off : nullptr;
+        a.post_shift = (d.flags & ISS_F_AFFINE_POST) ? blob + d.post_shift_off : nullptr;
+        a.flags = d.flags & ~ISS_F_SOFTMAX;
+        a.wt = Lr.wt;
+        a.N = d.cout;
+        if (d.kind == ISS_LAYER_DENSE) {
+            a.K = d.cin; a.H = 1; a.W = 1; a.C = d.cin; a.OH = 1; a.OW = 1;
+            a.KH = 1; a.KW = 1; a.SH = 1; a.SW = 1; a.PT = 0; a.PL = 0;
+        } else {
+            a.K = d.kh * d.kw * d.cin;
+            a.H = Lr.in_h; a.W = Lr.in_w; a.C = Lr.in_c; a.OH = Lr.out_h; a.OW = Lr.out_w;
+            a.KH = d.kh; a.KW = d.kw; a.SH = d.sh; a.SW = d.sw; a.PT = d.pad_top; a.PL = d.pad_left;
+        }
     }
-    if (j >= cnn->layers.size()) return false;
-    const Layer &Nx = cnn->layers[j];
-    ConvArgs probe = {};
-    fill_conv_args(Nx, nb, probe);
-    return f16_engine_covers(Nx, probe);
+    auto f16 = [&](const ConvArgs &a) { return iss_conv_is_f16(iss_conv_kernel(a, mode)); };
+    // does compute layer j run on engine 3 when handed split-half words?
+    auto reads_packed = [&](size_t j) { ConvArgs a = plan[j].a; a.in_packed = 1; return f16(a); };
+
+    bool packed = false;                                     // format of the activation the next layer reads
+    int pool_h = 0, pool_w = 0;                              // un-pooled dims of a pooling folded into the next layer
+    for (size_t li = 0; li < n; ++li) {
+        const Layer &Lr = cnn->layers[li];
+        const iss_layer_desc &d = Lr.d;
+        LayerPlan &P = plan[li];
+        if (d.kind == ISS_LAYER_MAXPOOL) {
+            ISS_REQUIRE(li > 0, ISS_ERR_UNSUPPORTED, "iss_cnn_forward: pooling as first layer is not supported");
+            // 2x2 / stride-2 'valid' pooling over split-half words in front of a convolution engine 3 takes with the
+            // pooling folded in: the maximum is taken in its operand fill (conv_gemm_tc.cu, LD_POOL)
+            const Layer *Nx = li + 1 < n ? &cnn->layers[li + 1] : nullptr;
+            if (packed && fuse_pool && (int)li != cnn->prof_layer && Nx && d.kh == 2 && d.kw == 2 && d.sh == 2 && d.sw == 2 &&
+                d.pad_top == 0 && d.pad_left == 0 && d.pad_bottom == 0 && d.pad_right == 0 &&
+                Nx->d.kind == ISS_LAYER_CONV2D && Nx->d.pad_bottom == 0 && Nx->d.pad_right == 0) {
+                ConvArgs a = plan[li + 1].a;
+                a.in_packed = 1; a.pool_h = Lr.in_h; a.pool_w = Lr.in_w;
+                if (f16(a)) { P.step = Step::FOLDED_POOL; pool_h = Lr.in_h; pool_w = Lr.in_w; continue; }
+            }
+            P.step = packed ? Step::POOL_PACKED : (Lr.in_c % 4 == 0 ? Step::POOL_VEC4 : Step::POOL);
+            continue;
+        }
+        ConvArgs &a = P.a;
+        a.in_packed = packed;
+        a.pool_h = pool_h; a.pool_w = pool_w;
+        pool_h = pool_w = 0;
+        // split-half output iff the next compute layer reads it on engine 3; pooling layers in between keep the
+        // format (the packed pooling kernel moves 4 channels per thread)
+        size_t j = li + 1;
+        bool pools_vec4 = true;
+        for (; j < n && cnn->layers[j].d.kind == ISS_LAYER_MAXPOOL; ++j) pools_vec4 = pools_vec4 && cnn->layers[j].in_c % 4 == 0;
+        const bool next_packed = j < n && pools_vec4 && reads_packed(j);
+        if (li == 0) {
+            ISS_REQUIRE(d.kind == ISS_LAYER_CONV2D, ISS_ERR_UNSUPPORTED, "iss_cnn_forward: first layer must be Conv2D");
+            const bool direct = d.cin == 1 && (d.cout == 16 || d.cout == 32 || d.cout == 64 || d.cout == 128) && !(d.flags & ISS_F_SOFTMAX);
+            P.step = direct ? Step::FIRST_DIRECT : Step::FIRST_GENERIC;
+            a.out_packed = direct && next_packed;            // the generic first layer writes fp32
+            // the fused first layer (FirstFuse, conv_gemm.cuh): the direct kernel's shape without padding / stride, in
+            // layer 1's slab-kernel operand fill
+            *fuse_first = false;
+            if (a.out_packed && fuse_first_on && first_map && d.sh == 1 && d.sw == 1 && d.pad_top == 0 && d.pad_left == 0 &&
+                d.pad_bottom == 0 && d.pad_right == 0 && !(d.flags & ISS_F_SIGMOID) && cnn->layers[1].d.kind == ISS_LAYER_CONV2D &&
+                cnn->layers[1].d.pad_bottom == 0 && cnn->layers[1].d.pad_right == 0) {
+                const FirstFuse probe = {};
+                ConvArgs a1 = plan[1].a;
+                a1.in_packed = 1; a1.first = &probe;
+                *fuse_first = f16(a1);
+            }
+        } else {
+            P.step = Step::CONV;
+            a.out_packed = next_packed && f16(a);
+        }
+        packed = a.out_packed;
+    }
+    return ISS_OK;
 }
 
 }  // namespace
@@ -628,6 +690,11 @@ extern "C" int iss_cnn_forward(iss_ctx *ctx, iss_cnn *cnn, const float *d_mspec,
     };
     bool ranges_ascending = true;
     for (int s = 1; s < n_seg; ++s) ranges_ascending = ranges_ascending && h_seg_start[s] >= h_seg_stop[s - 1];
+    const int mode = iss_get_gemm_mode();
+    std::vector<LayerPlan> plan;
+    bool fuse_first = false;
+    const int prc = plan_forward(cnn, mode, d_first_yh && ranges_ascending, plan, &fuse_first);
+    if (prc != ISS_OK) return prc;
     ISS_CUDA_OK(cudaMemcpyAsync(d_seg_start, h_seg_start, sizeof(int32_t) * n_seg, cudaMemcpyHostToDevice, st));
     ISS_CUDA_OK(cudaMemcpyAsync(d_seg_off, off.data(), sizeof(int64_t) * (n_seg + 1), cudaMemcpyHostToDevice, st));
 
@@ -636,19 +703,18 @@ extern "C" int iss_cnn_forward(iss_ctx *ctx, iss_cnn *cnn, const float *d_mspec,
     ISS_CUDA_OK(cudaGetLastError());
     iss_count_launch(2);
 
-    const float *blob = cnn->d_blob;
     const int K = cnn->n_classes;
     for (int64_t b0 = 0; b0 < n; b0 += B) {
         const int64_t nb = std::min<int64_t>(B, n - b0);
         const float *cur = nullptr;
         int which = 0;
-        bool cur_packed = false;                                 // format of `cur`: fp32 values or split-half words
-        FirstFuse ffuse = {};                                    // set by layer 0 when it is folded into layer 1's operand fill
+        FirstFuse ffuse = {};                                    // set by layer 0 when this batch folds it into layer 1
         bool first_fused = false;
-        int pend_pool_h = 0, pend_pool_w = 0;                    // un-pooled dims of a MaxPooling2D folded into the next convolution
         for (size_t li = 0; li < cnn->layers.size(); ++li) {
             const Layer &Lr = cnn->layers[li];
             const iss_layer_desc &d = Lr.d;
+            const LayerPlan &P = plan[li];
+            if (P.step == Step::FOLDED_POOL) continue;
             const bool last = (li + 1 == cnn->layers.size());
             float *dst = last ? (logits + b0 * K) : act[which];
             const bool prof = ((int)li == cnn->prof_layer);
@@ -662,31 +728,13 @@ extern "C" int iss_cnn_forward(iss_ctx *ctx, iss_cnn *cnn, const float *d_mspec,
                 }
                 ISS_CUDA_OK(cudaEventRecord(cnn->prof_ev[cnn->prof_used], st));
             }
-            if (d.kind == ISS_LAYER_MAXPOOL && cur_packed && li > 0 && li + 1 < cnn->layers.size()) {
-                // 2x2 / stride-2 'valid' pooling in front of a convolution the fp16-split engine takes: the maximum is taken in
-                // its operand fill (conv_gemm_tc.cu, LD_POOL) and this layer never runs.  ISS_B200_FUSE_POOL=0: A/B tests.
-                const char *pool_env = getenv("ISS_B200_FUSE_POOL");
-                const bool pool_off = pool_env && pool_env[0] == '0';
-                const Layer &Nx = cnn->layers[li + 1];
-                if (!pool_off && !prof && d.kh == 2 && d.kw == 2 && d.sh == 2 && d.sw == 2 && d.pad_top == 0 && d.pad_left == 0 &&
-                    d.pad_bottom == 0 && d.pad_right == 0 && Nx.d.kind == ISS_LAYER_CONV2D && Nx.d.pad_bottom == 0 && Nx.d.pad_right == 0 &&
-                    iss_get_gemm_mode() == ISS_GEMM_TC_F16) {
-                    ConvArgs pn = {};
-                    fill_conv_args(Nx, nb, pn);
-                    pn.in_packed = 1;
-                    pn.flags = Nx.d.flags & ~ISS_F_SOFTMAX;
-                    pn.pool_h = Lr.in_h; pn.pool_w = Lr.in_w;
-                    if (iss_conv_f16_covers(pn)) { pend_pool_h = Lr.in_h; pend_pool_w = Lr.in_w; continue; }
-                }
-            }
-            if (d.kind == ISS_LAYER_MAXPOOL) {
-                ISS_REQUIRE(li > 0, ISS_ERR_UNSUPPORTED, "iss_cnn_forward: pooling as first layer is not supported");
+            if (P.step == Step::POOL || P.step == Step::POOL_VEC4 || P.step == Step::POOL_PACKED) {
                 const int64_t total = nb * Lr.out_h * Lr.out_w * Lr.out_c;
-                if (cur_packed)                                   // (format kept: the consumer behind the pooling asked for words)
+                if (P.step == Step::POOL_PACKED)
                     maxpool_nhwc_packed_kernel<<<(unsigned)((total / 4 + 255) / 256), 256, 0, st>>>(
                         reinterpret_cast<const uint4 *>(cur), reinterpret_cast<uint4 *>(dst), total / 4, Lr.in_h, Lr.in_w, Lr.in_c / 4,
                         Lr.out_h, Lr.out_w, d.kh, d.kw, d.sh, d.sw, d.pad_top, d.pad_left);
-                else if (Lr.in_c % 4 == 0)
+                else if (P.step == Step::POOL_VEC4)
                     maxpool_nhwc_vec4_kernel<<<(unsigned)((total / 4 + 255) / 256), 256, 0, st>>>(
                         reinterpret_cast<const float4 *>(cur), reinterpret_cast<float4 *>(dst), total / 4, Lr.in_h, Lr.in_w, Lr.in_c / 4,
                         Lr.out_h, Lr.out_w, d.kh, d.kw, d.sh, d.sw, d.pad_top, d.pad_left);
@@ -696,42 +744,12 @@ extern "C" int iss_cnn_forward(iss_ctx *ctx, iss_cnn *cnn, const float *d_mspec,
                 ISS_CUDA_OK(cudaGetLastError());
                 iss_count_launch();
             } else {
-                ConvArgs a = {};
-                a.w = blob + d.w_off;
-                a.bias = (d.flags & ISS_F_BIAS) ? blob + d.bias_off : nullptr;
-                a.pre_scale = (d.flags & ISS_F_AFFINE_PRE) ? blob + d.pre_scale_off : nullptr;
-                a.pre_shift = (d.flags & ISS_F_AFFINE_PRE) ? blob + d.pre_shift_off : nullptr;
-                a.post_scale = (d.flags & ISS_F_AFFINE_POST) ? blob + d.post_scale_off : nullptr;
-                a.post_shift = (d.flags & ISS_F_AFFINE_POST) ? blob + d.post_shift_off : nullptr;
+                ConvArgs a = P.a;
                 a.out = dst;
-                a.flags = d.flags & ~ISS_F_SOFTMAX;
-                fill_conv_args(Lr, nb, a);
-                a.in_packed = cur_packed ? 1 : 0;
-                const bool direct = li == 0 && d.kind == ISS_LAYER_CONV2D && d.cin == 1 &&
-                                    (d.cout == 16 || d.cout == 32 || d.cout == 64 || d.cout == 128) && !(d.flags & ISS_F_SOFTMAX);
-                // only the direct first-layer kernel and the fp16-split engine can emit split-half words
-                const bool can_pack = direct || (li > 0 && iss_get_gemm_mode() == ISS_GEMM_TC_F16 && f16_engine_covers(Lr, a));
-                a.out_packed = (!last && can_pack && wants_packed_output(cnn, li, nb)) ? 1 : 0;
-                ISS_REQUIRE(!a.in_packed || (li > 0 && f16_engine_covers(Lr, a)), ISS_ERR_UNSUPPORTED,
-                            "iss_cnn_forward: layer %d was handed split-half words it cannot read", (int)li);
-                int rc;
-                // Fold the first layer into the next convolution's operand fill (FirstFuse, conv_gemm.cuh)?  Needs: the direct
-                // first-layer shape without padding / stride, an fp16-split convolution right behind it that takes it, and a
-                // batch whose patches span few enough frames for the float64 map.
-                const char *fuse_env = getenv("ISS_B200_FUSE_FIRST");      // "0" = keep the stand-alone first-layer kernel (A/B tests)
-                const bool fuse_off = fuse_env && fuse_env[0] == '0';
-                bool next_is_direct = false;                     // the fused first layer lives in the fp16-split engine only
-                if (li == 0 && cnn->layers.size() > 1 && cnn->layers[1].d.kind == ISS_LAYER_CONV2D &&
-                    cnn->layers[1].d.pad_bottom == 0 && cnn->layers[1].d.pad_right == 0 && iss_get_gemm_mode() == ISS_GEMM_TC_F16) {
-                    ConvArgs p1 = {};
-                    fill_conv_args(cnn->layers[1], nb, p1);
-                    p1.in_packed = 1;
-                    p1.flags = cnn->layers[1].d.flags & ~ISS_F_SOFTMAX;
-                    p1.first = &ffuse;
-                    next_is_direct = iss_conv_f16_covers(p1);
-                }
-                if (li == 0 && direct && a.out_packed && !fuse_off && d_first_yh && ranges_ascending && next_is_direct && d.sh == 1 && d.sw == 1 && d.pad_top == 0 && d.pad_left == 0 &&
-                    d.pad_bottom == 0 && d.pad_right == 0 && !(d.flags & (ISS_F_SOFTMAX | ISS_F_SIGMOID))) {
+                a.M = nb * a.OH * a.OW;
+                int rc = ISS_OK;
+                if (li == 0 && fuse_first) {
+                    // the float64 map of the first layer covers the frames this batch's patches span, if few enough
                     const int64_t f_first = host_row0(b0), f_last = host_row0(b0 + nb - 1);
                     const int64_t rows = f_last - f_first + Lr.out_h;
                     if (rows <= first_y_rows(B)) {
@@ -745,44 +763,34 @@ extern "C" int iss_cnn_forward(iss_ctx *ctx, iss_cnn *cnn, const float *d_mspec,
                         ffuse.Yh = d_first_yh; ffuse.Yl = d_first_yl; ffuse.y_f0 = f_first; ffuse.y_rows = rows;
                         ffuse.row0 = pa.row0 + b0; ffuse.coef = d_first_coef;
                         ffuse.post_scale = a.post_scale; ffuse.post_shift = a.post_shift; ffuse.flags = a.flags; ffuse.n_img = nb;
-                        first_fused = true;
+                        first_fused = true;                      // nothing stored: layer 1 reads the map
                     }
                 }
-                if (li == 0 && first_fused) {
-                    rc = ISS_OK;                                  // nothing stored: layer 1 reads the map
-                } else if (li == 0) {
-                    ISS_REQUIRE(d.kind == ISS_LAYER_CONV2D, ISS_ERR_UNSUPPORTED, "iss_cnn_forward: first layer must be Conv2D");
-                    if (direct) {
-                        FirstArgs f = {};
-                        f.mspec = d_mspec; f.ld = ld; f.row0 = pa.row0 + b0; f.mu = pa.mu + b0; f.sigma = pa.sigma + b0;
-                        f.w = a.w; f.bias = a.bias; f.pre_scale = a.pre_scale; f.pre_shift = a.pre_shift;
-                        f.post_scale = a.post_scale; f.post_shift = a.post_shift; f.out = dst; f.n = nb;
-                        f.H = Lr.in_h; f.W = Lr.in_w; f.OH = Lr.out_h; f.OW = Lr.out_w; f.KH = d.kh; f.KW = d.kw;
-                        f.SH = d.sh; f.SW = d.sw; f.PT = d.pad_top; f.PL = d.pad_left;
-                        f.Hp = Lr.in_h + d.pad_top + d.pad_bottom; f.Wp = Lr.in_w + d.pad_left + d.pad_right;
-                        f.Cout = d.cout; f.flags = a.flags; f.out_packed = a.out_packed;
-                        const size_t smem = ((size_t)d.kh * d.kw * d.cout + (size_t)f.Hp * f.Wp + FIRST_P * d.sw + d.kw + 8) * sizeof(float);
-                        ISS_REQUIRE(smem <= 200 * 1024, ISS_ERR_UNSUPPORTED, "iss_cnn_forward: first layer too large for the first-layer kernel");
-                        ISS_CUDA_OK(iss_optin_smem(reinterpret_cast<const void *>(conv_first_direct_kernel), 200 * 1024));
-                        const unsigned grid = (unsigned)std::min<int64_t>(nb, (int64_t)ctx->sm_count * 8);
-                        conv_first_direct_kernel<<<grid, 256, smem, st>>>(f);
-                        ISS_CUDA_OK(cudaGetLastError());
-                        iss_count_launch();
-                        rc = ISS_OK;
-                    } else {
-                        a.in = d_mspec; a.ld = ld; a.row0 = pa.row0 + b0; a.mu = pa.mu + b0; a.sigma = pa.sigma + b0;
-                        a.out_packed = 0;                         // the generic first-layer kernel writes fp32
-                        rc = iss_launch_conv(a, true, st);
-                    }
-                } else {
+                if (P.step == Step::FIRST_DIRECT && !first_fused) {
+                    FirstArgs f = {};
+                    f.mspec = d_mspec; f.ld = ld; f.row0 = pa.row0 + b0; f.mu = pa.mu + b0; f.sigma = pa.sigma + b0;
+                    f.w = a.w; f.bias = a.bias; f.pre_scale = a.pre_scale; f.pre_shift = a.pre_shift;
+                    f.post_scale = a.post_scale; f.post_shift = a.post_shift; f.out = dst; f.n = nb;
+                    f.H = Lr.in_h; f.W = Lr.in_w; f.OH = Lr.out_h; f.OW = Lr.out_w; f.KH = d.kh; f.KW = d.kw;
+                    f.SH = d.sh; f.SW = d.sw; f.PT = d.pad_top; f.PL = d.pad_left;
+                    f.Hp = Lr.in_h + d.pad_top + d.pad_bottom; f.Wp = Lr.in_w + d.pad_left + d.pad_right;
+                    f.Cout = d.cout; f.flags = a.flags; f.out_packed = a.out_packed;
+                    const size_t smem = ((size_t)d.kh * d.kw * d.cout + (size_t)f.Hp * f.Wp + FIRST_P * d.sw + d.kw + 8) * sizeof(float);
+                    ISS_REQUIRE(smem <= 200 * 1024, ISS_ERR_UNSUPPORTED, "iss_cnn_forward: first layer too large for the first-layer kernel");
+                    ISS_CUDA_OK(iss_optin_smem(reinterpret_cast<const void *>(conv_first_direct_kernel), 200 * 1024));
+                    const unsigned grid = (unsigned)std::min<int64_t>(nb, (int64_t)ctx->sm_count * 8);
+                    conv_first_direct_kernel<<<grid, 256, smem, st>>>(f);
+                    ISS_CUDA_OK(cudaGetLastError());
+                    iss_count_launch();
+                } else if (P.step == Step::FIRST_GENERIC) {
+                    a.in = d_mspec; a.ld = ld; a.row0 = pa.row0 + b0; a.mu = pa.mu + b0; a.sigma = pa.sigma + b0;
+                    rc = iss_launch_conv(a, mode, st);
+                } else if (P.step == Step::CONV) {
                     a.in = cur;
-                    a.pool_h = pend_pool_h; a.pool_w = pend_pool_w;
-                    pend_pool_h = pend_pool_w = 0;
-                    if (li == 1 && first_fused) { a.first = &ffuse; a.in = nullptr; a.in_packed = 1; }
-                    rc = iss_launch_conv(a, false, st);
+                    if (li == 1 && first_fused) { a.first = &ffuse; a.in = nullptr; }
+                    rc = iss_launch_conv(a, mode, st);
                 }
                 if (rc != ISS_OK) return rc;
-                cur_packed = a.out_packed != 0;
             }
             if (prof) {
                 ISS_CUDA_OK(cudaEventRecord(cnn->prof_ev[cnn->prof_used + 1], st));

@@ -246,18 +246,40 @@ int launch_conv_t(const ConvArgs &a, cudaStream_t st)
 
 }  // namespace
 
-int iss_launch_conv(const ConvArgs &a, bool first, cudaStream_t st)
+IssConvKernel iss_conv_kernel(const ConvArgs &a, int mode)
 {
-    if (!first && small_n_covers(a)) {
+    if (a.row0) return ISS_CONV_F32_FIRST;
+    if (small_n_covers(a)) return ISS_CONV_SMALL_N;
+    if (mode == ISS_GEMM_FP32 || !a.wt.tiled) return ISS_CONV_F32;
+    if (mode == ISS_GEMM_TC_F16 && a.wt.f16 && !(a.flags & ISS_F_SIGMOID)) {
+        const bool slab = iss_slab_covers(a);
+        // folded pooling: 2x2 / stride-2 'valid' over split-half words, in the gather kernel's operand fill
+        const bool pool_ok = a.pool_h == 0 || (!a.first && a.in_packed && a.pool_h / 2 == a.H && a.pool_w / 2 == a.W);
+        // the fused first layer: in the slab kernel's operand fill
+        const bool first_ok = !a.first || (slab && !(a.flags & ISS_F_RESIDUAL));
+        if (pool_ok && first_ok) return slab ? ISS_CONV_F16_SLAB : ISS_CONV_F16;
+    }
+    return ISS_CONV_TF32;
+}
+
+int iss_launch_conv(const ConvArgs &a, int mode, cudaStream_t st)
+{
+    const IssConvKernel k = iss_conv_kernel(a, mode);
+    ISS_REQUIRE(iss_conv_is_f16(k) || (!a.in_packed && !a.out_packed && !a.residual_packed && !a.first && a.pool_h == 0), ISS_ERR_UNSUPPORTED,
+                "conv: split-half tensors, folded pooling and the fused first layer need the fp16-split engine");
+    switch (k) {
+    case ISS_CONV_F32_FIRST: return launch_conv_t<true>(a, st);
+    case ISS_CONV_SMALL_N: {
         const int64_t gm = (a.M + 7) / 8;
         dense_small_n_kernel<<<(unsigned)(gm < 132 * 8 ? gm : 132 * 8), 256, (size_t)a.K * a.N * sizeof(float), st>>>(a);
         ISS_CUDA_OK(cudaGetLastError());
         iss_count_launch();
         return ISS_OK;
     }
-    if (!first) {
-        const int mode = iss_get_gemm_mode();
-        if (mode != ISS_GEMM_FP32 && iss_conv_tc_eligible(a)) return iss_launch_conv_tc(a, mode, st);
+    case ISS_CONV_TF32: return iss_launch_conv_tf32(a, st);
+    case ISS_CONV_F16: return iss_launch_conv_f16(a, st);
+    case ISS_CONV_F16_SLAB: return iss_launch_conv_slab(a, st);
+    case ISS_CONV_F32: break;
     }
-    return first ? launch_conv_t<true>(a, st) : launch_conv_t<false>(a, st);
+    return launch_conv_t<false>(a, st);
 }

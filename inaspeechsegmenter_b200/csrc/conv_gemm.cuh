@@ -63,8 +63,16 @@ struct FirstFuse {
     int64_t n_img;                  // patches in the batch
 };
 
+// A layer's weights as the tensor-core engines' operand images (conv_gemm_tc.cu), owned by the layer.  An image that
+// is nullptr keeps the layer off that engine.
+struct TcWeights {
+    void *tiled = nullptr;          // engine 2: 3xTF32 hi / lo, tiled and swizzled as the shared-memory operand stages
+    void *f16 = nullptr;            // engine 3: fp16 hi / lo, likewise, pre-scaled by a power of two
+    float f16_inv_scale = 1.f;      // undoes that scale in the epilogue
+};
+
 struct ConvArgs {
-    const float *in;        // NHWC activations, or the log-mel rows when `first`
+    const float *in;        // NHWC activations, or the log-mel rows of the generic first layer
     const float *w;         // [K][N]
     const float *bias, *pre_scale, *pre_shift, *post_scale, *post_shift;
     const float *residual;  // [M][N] or nullptr
@@ -75,14 +83,12 @@ struct ConvArgs {
     int OH, OW;
     int KH, KW, SH, SW, PT, PL;
     int flags;
-    // `first` (sliding z-normalised patches of the segmenter CNNs) only
+    // generic first layer of the segmenter CNNs only (row0 != nullptr): gather the sliding patches from the log-mel
+    // rows `in` (row stride ld) and z-normalise them on the fly
     int ld;
     const int32_t *row0; const float *mu; const float *sigma;
-    // tensor-core path: weights transposed + split, [N][Kp] each (nullptr => fp32 CUDA-core kernel)
-    const float *wt_hi; const float *wt_lo; const float *wt_tiled; int Kp;
-    // fp16-split engine (engine 3, conv_gemm_tc.cu): tiled fp16 hi/lo weight image (nullptr => not prepared) and its scale
-    const void *wt_f16; float wt_f16_inv_scale;
-    // activation formats of that engine: fp32 values (0) or split-half words lo16 << 16 | hi16 (1)
+    TcWeights wt;
+    // activation formats of engine 3: fp32 values (0) or split-half words lo16 << 16 | hi16 (1)
     int in_packed, out_packed;
     int residual_packed;    // `residual` holds split-half words (fp16-split kernels only)
     int pool_h, pool_w;     // engine 3 only, > 0: `in` is the un-pooled [n][pool_h][pool_w][C] tensor, 2x2 / stride-2 max taken in the operand fill
@@ -97,16 +103,31 @@ struct ConvArgs {
 #endif
 
 extern "C" int iss_get_gemm_mode(void);
-bool iss_conv_tc_eligible(const ConvArgs &a);
-int iss_launch_conv_tc(const ConvArgs &a, int mode, cudaStream_t st);
-// W[K][N] -> device buffer: [2][N][Kp] row-major (hi, lo) then the tiled/pre-swizzled image [2*N*Kp]; Kp = K rounded up to 32
-int iss_prepare_tc_weights(const float *h_w, int K, int N, float **d_out, int *Kp_out);
-// W[K][N] -> fp16 hi/lo image of engine 3 (*d_out stays nullptr when the shape is not one that engine takes)
-int iss_prepare_f16_weights(const float *h_w, int K, int N, void **d_out, float *inv_scale);
-// does engine 3 take this layer (weight image, channel counts, the input format / folded pooling / fused first layer)?
-bool iss_conv_f16_covers(const ConvArgs &a);
-// n-tile width of engine 3 for N output channels (must agree between the weight image and the launch)
-int iss_f16_bn_for(int N);
 
-// Launches the layer on `st`.  first = gather from log-mel rows with (x - mu) / sigma.
-int iss_launch_conv(const ConvArgs &a, bool first, cudaStream_t st);
+// Builds the tensor-core images of the weights W[K][N] (Keras / blob layout) of a layer with C input channels: engine 2's
+// when C, K and N are multiples of 32, and engine 3's when `f16` is set and C and N are also multiples of 64.  These are
+// the only shape rules of the two engines.  On failure the images already built stay in *w for iss_free_weights.
+int iss_prepare_weights(const float *h_w, int C, int K, int N, bool f16, TcWeights *w);
+void iss_free_weights(TcWeights *w);
+
+// The kernel that runs a layer.  Only the engine-3 kernels (iss_conv_is_f16) read or write split-half words, take a
+// folded pooling (pool_h > 0) or the fused first layer (`first`).
+enum IssConvKernel {
+    ISS_CONV_F32,           // fp32 CUDA cores (conv_gemm.cu)
+    ISS_CONV_F32_FIRST,     // the same, gathering the generic first layer's patches from the log-mel rows
+    ISS_CONV_SMALL_N,       // fp32 dense / 1x1 layer with at most 8 outputs (the softmax heads)
+    ISS_CONV_TF32,          // engine 2, gather kernel
+    ISS_CONV_F16,           // engine 3, gather kernel
+    ISS_CONV_F16_SLAB,      // engine 3, slab kernel
+};
+inline bool iss_conv_is_f16(IssConvKernel k) { return k == ISS_CONV_F16 || k == ISS_CONV_F16_SLAB; }
+IssConvKernel iss_conv_kernel(const ConvArgs &a, int mode);
+
+// the tensor-core launchers behind iss_launch_conv (conv_gemm_tc.cu)
+bool iss_slab_covers(const ConvArgs &a);
+int iss_launch_conv_tf32(const ConvArgs &a, cudaStream_t st);
+int iss_launch_conv_f16(const ConvArgs &a, cudaStream_t st);
+int iss_launch_conv_slab(const ConvArgs &a, cudaStream_t st);
+
+// Launches the layer on `st` with the kernel iss_conv_kernel(a, mode) picks.
+int iss_launch_conv(const ConvArgs &a, int mode, cudaStream_t st);

@@ -594,15 +594,6 @@ conv_slab_kernel(const ConvArgs a, const FirstFuse ff, const unsigned char *__re
     }
 }
 
-// Does the slab kernel take this engine-3 layer?  Un-padded, stride-1 'valid' convolution, 64 -> 64 channels, no
-// folded pooling, and one slab plus a four-stage weight ring fit in shared memory.
-bool slab_covers(const ConvArgs &a)
-{
-    return a.wt_f16 && !(a.flags & ISS_F_SIGMOID) && a.C == SLAB_C && a.N == SLAB_N && a.K == a.KH * a.KW * a.C && a.pool_h == 0 &&
-           a.SH == 1 && a.SW == 1 && a.PT == 0 && a.PL == 0 && a.OH == a.H - a.KH + 1 && a.OW == a.W - a.KW + 1 &&
-           slab_smem(slab_rows(a.KH, a.KW, a.W), 1, SLAB_MAX_STAGES) <= SLAB_MAX_SMEM;
-}
-
 template <int MODE>
 int launch_slab(const ConvArgs &a, cudaStream_t st)
 {
@@ -621,7 +612,7 @@ int launch_slab(const ConvArgs &a, cudaStream_t st)
     ISS_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     const unsigned grid = (unsigned)(tiles < sms ? tiles : sms);
     const FirstFuse ff = a.first ? *a.first : FirstFuse{};
-    kern<<<grid, SLAB_THREADS, smem, st>>>(a, ff, reinterpret_cast<const unsigned char *>(a.wt_f16), a.wt_f16_inv_scale, rows,
+    kern<<<grid, SLAB_THREADS, smem, st>>>(a, ff, reinterpret_cast<const unsigned char *>(a.wt.f16), a.wt.f16_inv_scale, rows,
                                            tiles, nbuf, stages);
     ISS_CUDA_OK(cudaGetLastError());
     iss_count_launch();
@@ -631,19 +622,61 @@ int launch_slab(const ConvArgs &a, cudaStream_t st)
 template <int BN>
 int launch_f16(const ConvArgs &a, cudaStream_t st)
 {
-    const float s = a.wt_f16_inv_scale;
-    if (slab_covers(a)) {
-        if (a.first) return launch_slab<LD_FIRST>(a, st);
-        return a.in_packed ? launch_slab<LD_PACKED>(a, st) : launch_slab<LD_F32>(a, st);
-    }
-    if (a.pool_h > 0) return launch_wg<ENG_F16, BN, LD_POOL>(a, a.wt_f16, s, st);
-    if (a.in_packed) return launch_wg<ENG_F16, BN, LD_PACKED>(a, a.wt_f16, s, st);
-    return launch_wg<ENG_F16, BN, LD_F32>(a, a.wt_f16, s, st);
+    const float s = a.wt.f16_inv_scale;
+    if (a.pool_h > 0) return launch_wg<ENG_F16, BN, LD_POOL>(a, a.wt.f16, s, st);
+    if (a.in_packed) return launch_wg<ENG_F16, BN, LD_PACKED>(a, a.wt.f16, s, st);
+    return launch_wg<ENG_F16, BN, LD_F32>(a, a.wt.f16, s, st);
+}
+
+// n-tile width of engine 3: 128 output channels per CTA when N allows it, else 64 (the weight image and the launch agree)
+int f16_bn_for(int N) { return N % 128 == 0 ? 128 : 64; }
+
+// n-tile width of engine 2
+int tf32_bn_for(int N) { return N % 128 == 0 ? 128 : (N % 64 == 0 ? 64 : 32); }
+
+int upload(const void *h, size_t bytes, void **d_out, const char *what)
+{
+    void *d = nullptr;
+    cudaError_t e = cudaMalloc(&d, bytes);
+    if (e != cudaSuccess) { iss_set_error("cudaMalloc %s: %s", what, cudaGetErrorString(e)); return ISS_ERR_NOMEM; }
+    e = cudaMemcpy(d, h, bytes, cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) { cudaFree(d); iss_set_error("cudaMemcpy %s: %s", what, cudaGetErrorString(e)); return ISS_ERR_CUDA; }
+    *d_out = d;
+    return ISS_OK;
 }
 
 int g_gemm_mode = -1;      // -1 = read ISS_B200_GEMM on first use
 
 }  // namespace
+
+// Does the slab kernel take this engine-3 layer?  Un-padded, stride-1 'valid' convolution, 64 -> 64 channels, no
+// folded pooling, and one slab plus a four-stage weight ring fit in shared memory.
+bool iss_slab_covers(const ConvArgs &a)
+{
+    return a.C == SLAB_C && a.N == SLAB_N && a.K == a.KH * a.KW * a.C && a.pool_h == 0 &&
+           a.SH == 1 && a.SW == 1 && a.PT == 0 && a.PL == 0 && a.OH == a.H - a.KH + 1 && a.OW == a.W - a.KW + 1 &&
+           slab_smem(slab_rows(a.KH, a.KW, a.W), 1, SLAB_MAX_STAGES) <= SLAB_MAX_SMEM;
+}
+
+int iss_launch_conv_slab(const ConvArgs &a, cudaStream_t st)
+{
+    if (a.first) return launch_slab<LD_FIRST>(a, st);
+    return a.in_packed ? launch_slab<LD_PACKED>(a, st) : launch_slab<LD_F32>(a, st);
+}
+
+int iss_launch_conv_f16(const ConvArgs &a, cudaStream_t st)
+{
+    return f16_bn_for(a.N) == 128 ? launch_f16<128>(a, st) : launch_f16<64>(a, st);
+}
+
+int iss_launch_conv_tf32(const ConvArgs &a, cudaStream_t st)
+{
+    switch (tf32_bn_for(a.N)) {
+    case 128: return launch_wg<ENG_TF32, 128, LD_F32>(a, a.wt.tiled, 1.f, st);
+    case 64: return launch_wg<ENG_TF32, 64, LD_F32>(a, a.wt.tiled, 1.f, st);
+    default: return launch_wg<ENG_TF32, 32, LD_F32>(a, a.wt.tiled, 1.f, st);
+    }
+}
 
 extern "C" int iss_set_gemm_mode(int mode)
 {
@@ -664,98 +697,46 @@ extern "C" int iss_get_gemm_mode(void)
     return g_gemm_mode;
 }
 
-bool iss_conv_tc_eligible(const ConvArgs &a)
+// Engine 2's image: [N/BN][K/32][hi | lo][BN rows x 32 floats], the 16-byte chunk j of row n stored at chunk j ^ (n & 7)
+// (one cp.async stage per k-block).  Engine 3's: [N/BN][K/64][hi | lo][BN rows x 64 halves] in the same swizzle
+// (f16_image.cuh), pre-scaled by a power of two.
+int iss_prepare_weights(const float *h_w, int C, int K, int N, bool f16, TcWeights *w)
 {
-    return a.wt_hi && a.wt_lo && a.wt_tiled && a.Kp > 0 && a.C % 32 == 0 && a.K % 32 == 0 && a.N % 32 == 0 && a.N >= 32;
-}
-
-// n-tile width of engine 3: 128 output channels per CTA when N allows it, else 64
-int iss_f16_bn_for(int N) { return N % 128 == 0 ? 128 : 64; }
-
-bool iss_conv_f16_covers(const ConvArgs &a)
-{
-    if (!a.wt_f16 || (a.flags & ISS_F_SIGMOID)) return false;
-    if (a.C % HBK != 0 || a.N % 64 != 0 || a.K != a.KH * a.KW * a.C) return false;
-    if (a.pool_h > 0 && (a.first || !a.in_packed || a.pool_h / 2 != a.H || a.pool_w / 2 != a.W)) return false;   // 2x2 / stride-2 'valid' pooling only
-    if (a.first && (!slab_covers(a) || (a.flags & ISS_F_RESIDUAL))) return false;    // the fused first layer runs in the slab kernel
-    return true;
-}
-
-int iss_launch_conv_tc(const ConvArgs &a, int mode, cudaStream_t st)
-{
-    if (mode == ISS_GEMM_TC_F16 && iss_conv_f16_covers(a))
-        return iss_f16_bn_for(a.N) == 128 ? launch_f16<128>(a, st) : launch_f16<64>(a, st);
-    ISS_REQUIRE(!a.in_packed && !a.out_packed && !a.residual_packed && !a.first && a.pool_h == 0, ISS_ERR_UNSUPPORTED,
-                "conv_tc: split-half tensors, folded pooling and the fused first layer need the fp16-split engine");
-    if (a.N % 128 == 0) return launch_wg<ENG_TF32, 128, LD_F32>(a, a.wt_tiled, 1.f, st);
-    if (a.N % 64 == 0) return launch_wg<ENG_TF32, 64, LD_F32>(a, a.wt_tiled, 1.f, st);
-    return launch_wg<ENG_TF32, 32, LD_F32>(a, a.wt_tiled, 1.f, st);
-}
-
-static int tc_block_n(int N) { return N % 128 == 0 ? 128 : (N % 64 == 0 ? 64 : 32); }
-
-// Host-side preparation of a layer's weights for engine 2:
-// W[K][N] (Keras / our blob layout) ->
-//   (1) transposed, zero-padded, split row-major [2][N][Kp], followed by
-//   (2) the same values tiled and pre-swizzled as smem operand images
-//       [N/BN][Kp/32][hi|lo][BN rows x 128 B, 16-byte chunk j of row n stored at chunk j ^ (n & 7)]
-//       (one cp.async stage per k-block).
-int iss_prepare_tc_weights(const float *h_w, int K, int N, float **d_out, int *Kp_out)
-{
-    const int Kp = (K + TBK - 1) / TBK * TBK;
-    const size_t plane = (size_t)N * Kp;
-    std::vector<float> buf(4 * plane, 0.f);
-    float *hi = buf.data(), *lo = buf.data() + plane, *tiled = buf.data() + 2 * plane;
-    for (int k = 0; k < K; ++k)
-        for (int n = 0; n < N; ++n) {
-            const float w = h_w[(size_t)k * N + n];
-            uint32_t u;
-            memcpy(&u, &w, 4);
-            u &= 0xFFFFE000u;
-            float h;
-            memcpy(&h, &u, 4);
-            hi[(size_t)n * Kp + k] = h;
-            lo[(size_t)n * Kp + k] = w - h;
-        }
-    const int BN = tc_block_n(N), nkb = Kp / TBK;
-    for (int nt = 0; nt < N / BN; ++nt)
-        for (int kb = 0; kb < nkb; ++kb)
-            for (int part = 0; part < 2; ++part) {
-                float *dst = tiled + (((size_t)nt * nkb + kb) * 2 + part) * (size_t)BN * TBK;
-                const float *src = part ? lo : hi;
-                for (int n = 0; n < BN; ++n)
-                    for (int k = 0; k < TBK; ++k) {
-                        const int chunk = (k >> 2) ^ (n & 7);
-                        dst[n * TBK + chunk * 4 + (k & 3)] = src[(size_t)(nt * BN + n) * Kp + kb * TBK + k];
-                    }
-            }
-    float *d = nullptr;
-    cudaError_t e = cudaMalloc(&d, buf.size() * sizeof(float));
-    if (e != cudaSuccess) { iss_set_error("cudaMalloc tc weights: %s", cudaGetErrorString(e)); return ISS_ERR_NOMEM; }
-    e = cudaMemcpy(d, buf.data(), buf.size() * sizeof(float), cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) { cudaFree(d); iss_set_error("cudaMemcpy tc weights: %s", cudaGetErrorString(e)); return ISS_ERR_CUDA; }
-    *d_out = d;
-    *Kp_out = Kp;
-    return ISS_OK;
-}
-
-// Host-side preparation of a layer's weights for engine 3: W[K][N] (Keras / blob layout) -> device image
-// [n-tile][k-block of 64][hi | lo][BN rows x 128 B, SWIZZLE_128B] of fp16 halves, pre-scaled by a power of two
-// (undone in the epilogue with *inv_scale).  Owned by the layer (freed with cudaFree by its destructor).
-int iss_prepare_f16_weights(const float *h_w, int K, int N, void **d_out, float *inv_scale)
-{
-    *d_out = nullptr; *inv_scale = 1.f;
-    if (K % HBK != 0 || N % 64 != 0) return ISS_OK;             // not a shape this engine takes
-    std::vector<float> wt((size_t)N * K, 0.f);                   // transposed [N][K]
+    *w = TcWeights{};
+    if (C % 32 != 0 || K % 32 != 0 || N % 32 != 0) return ISS_OK;
+    std::vector<float> wt((size_t)N * K);                         // transposed [N][K]
     for (int k = 0; k < K; ++k)
         for (int n = 0; n < N; ++n) wt[(size_t)n * K + k] = h_w[(size_t)k * N + n];
+    const int BN = tf32_bn_for(N), nkb = K / TBK;
+    std::vector<float> tiled((size_t)2 * N * K);
+    for (int nt = 0; nt < N / BN; ++nt)
+        for (int kb = 0; kb < nkb; ++kb) {
+            float *hi = tiled.data() + ((size_t)nt * nkb + kb) * 2 * BN * TBK, *lo = hi + BN * TBK;
+            for (int n = 0; n < BN; ++n)
+                for (int k = 0; k < TBK; ++k) {
+                    const float x = wt[(size_t)(nt * BN + n) * K + kb * TBK + k];
+                    uint32_t u;
+                    memcpy(&u, &x, 4);
+                    u &= 0xFFFFE000u;
+                    float h;
+                    memcpy(&h, &u, 4);
+                    const int o = n * TBK + (((k >> 2) ^ (n & 7)) << 2) + (k & 3);
+                    hi[o] = h;
+                    lo[o] = x - h;
+                }
+        }
+    int rc = upload(tiled.data(), tiled.size() * sizeof(float), &w->tiled, "tc weights");
+    if (rc != ISS_OK || !f16 || C % 64 != 0 || N % 64 != 0) return rc;
     std::vector<__half> img;
-    const float scale = iss_f16_build_image(wt.data(), N, K, K, iss_f16_bn_for(N), img);
-    void *d = nullptr;
-    cudaError_t e = cudaMalloc(&d, img.size() * sizeof(__half));
-    if (e != cudaSuccess) { iss_set_error("cudaMalloc f16 weights: %s", cudaGetErrorString(e)); return ISS_ERR_NOMEM; }
-    e = cudaMemcpy(d, img.data(), img.size() * sizeof(__half), cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) { cudaFree(d); iss_set_error("cudaMemcpy f16 weights: %s", cudaGetErrorString(e)); return ISS_ERR_CUDA; }
-    *d_out = d; *inv_scale = 1.f / scale;
-    return ISS_OK;
+    const float scale = iss_f16_build_image(wt.data(), N, K, K, f16_bn_for(N), img);
+    rc = upload(img.data(), img.size() * sizeof(__half), &w->f16, "f16 weights");
+    if (rc == ISS_OK) w->f16_inv_scale = 1.f / scale;
+    return rc;
+}
+
+void iss_free_weights(TcWeights *w)
+{
+    if (w->tiled) cudaFree(w->tiled);
+    if (w->f16) cudaFree(w->f16);
+    *w = TcWeights{};
 }

@@ -25,10 +25,7 @@ namespace {
 struct RConv {
     int kh, kw, stride, pad, cin, cout;
     int64_t w_off, scale_off, shift_off;
-    float *d_wt = nullptr;      // tensor-core weights [2][N][Kp]
-    int Kp = 0;
-    void *d_wt_f16 = nullptr;   // fp16 hi/lo image of engine 3 (cin % 64 == 0 && cout % 64 == 0: every conv of stages 2-4)
-    float f16_inv_scale = 1.f;
+    TcWeights wt;
 };
 
 struct RBlock {
@@ -79,8 +76,7 @@ struct iss_resnet {
     std::vector<RBlock> blocks;
     int64_t emb_w_off, emb_b_off;
     int c_final, h_final;
-    float *d_emb_wt = nullptr;
-    int emb_Kp = 0;
+    TcWeights emb_wt;
 };
 
 namespace {
@@ -187,14 +183,7 @@ extern "C" int iss_resnet_create(iss_ctx *ctx, const float *h_blob, int64_t blob
     if (e != cudaSuccess) { delete net; iss_set_error("cudaMalloc resnet blob: %s", cudaGetErrorString(e)); return ISS_ERR_NOMEM; }
     e = cudaMemcpy(net->d_blob, h_blob, (size_t)blob_len * sizeof(float), cudaMemcpyHostToDevice);
     if (e != cudaSuccess) { cudaFree(net->d_blob); delete net; iss_set_error("cudaMemcpy resnet blob: %s", cudaGetErrorString(e)); return ISS_ERR_CUDA; }
-    auto prep = [&](RConv &c) -> int {
-        const int K = c.kh * c.kw * c.cin;
-        if (c.cin % 32 != 0 || K % 32 != 0 || c.cout % 32 != 0) return ISS_OK;
-        const int rc = iss_prepare_tc_weights(h_blob + c.w_off, K, c.cout, &c.d_wt, &c.Kp);
-        // fp16-split image: 64-channel k-blocks, 64-wide n-tiles
-        if (rc != ISS_OK || c.cin % 64 != 0 || c.cout % 64 != 0) return rc;
-        return iss_prepare_f16_weights(h_blob + c.w_off, K, c.cout, &c.d_wt_f16, &c.f16_inv_scale);
-    };
+    auto prep = [&](RConv &c) { return iss_prepare_weights(h_blob + c.w_off, c.cin, c.kh * c.kw * c.cin, c.cout, true, &c.wt); };
     int prc = ISS_OK;
     for (RBlock &b : net->blocks) {
         if (prc == ISS_OK) prc = prep(b.c1);
@@ -203,8 +192,9 @@ extern "C" int iss_resnet_create(iss_ctx *ctx, const float *h_blob, int64_t blob
         if (prc == ISS_OK && b.has_sc) prc = prep(b.sc);
     }
     if (prc == ISS_OK) {
+        // the embedding stays on engine 2 in every mode: no engine-3 image
         const int K = 2 * net->c_final * net->h_final;
-        prc = iss_prepare_tc_weights(h_blob + net->emb_w_off, K, net->embed_dim, &net->d_emb_wt, &net->emb_Kp);
+        prc = iss_prepare_weights(h_blob + net->emb_w_off, K, K, net->embed_dim, false, &net->emb_wt);
     }
     if (prc != ISS_OK) { iss_resnet_destroy(net); return prc; }
     *out = net;
@@ -216,14 +206,9 @@ extern "C" int iss_resnet_destroy(iss_resnet *net)
     if (!net) return ISS_OK;
     cudaSetDevice(net->ctx->device);
     if (net->d_blob) cudaFree(net->d_blob);
-    if (net->d_emb_wt) cudaFree(net->d_emb_wt);
-    for (RBlock &b : net->blocks) {
-        for (RConv *c : {&b.c1, &b.c2, &b.c3, &b.sc}) {
-            if (c == &b.sc && !b.has_sc) continue;
-            if (c->d_wt) cudaFree(c->d_wt);
-            if (c->d_wt_f16) cudaFree(c->d_wt_f16);
-        }
-    }
+    iss_free_weights(&net->emb_wt);
+    for (RBlock &b : net->blocks)
+        for (RConv *c : {&b.c1, &b.c2, &b.c3, &b.sc}) iss_free_weights(&c->wt);
     delete net;
     return ISS_OK;
 }
@@ -278,23 +263,29 @@ extern "C" int iss_resnet_embed(iss_ctx *ctx, iss_resnet *net, const float *d_fe
     ISS_CUDA_OK(cudaMemcpyAsync(d_start, h_win_start, sizeof(int32_t) * n_windows, cudaMemcpyHostToDevice, st));
     const float *blob = net->d_blob;
 
+    // the filter shape and weights of a convolution (the batch, the spatial dims and the tensors are set per launch)
+    auto conv_args = [&](const RConv &c) {
+        ConvArgs a = {};
+        a.w = blob + c.w_off; a.pre_scale = blob + c.scale_off; a.pre_shift = blob + c.shift_off;
+        a.wt = c.wt;
+        a.N = c.cout; a.K = c.kh * c.kw * c.cin; a.C = c.cin;
+        a.KH = c.kh; a.KW = c.kw; a.SH = c.stride; a.SW = c.stride; a.PT = c.pad; a.PL = c.pad;
+        a.flags = ISS_F_AFFINE_PRE;
+        return a;
+    };
     // Activation formats (conv_gemm.cuh): a tensor is stored as split-half words when its producer AND every consumer run on
-    // the fp16-split engine (all convolutions with cin % 64 == 0 and cout % 64 == 0, i.e. stages 2-4), fp32 otherwise.
-    const bool f16_mode = iss_get_gemm_mode() == ISS_GEMM_TC_F16;
-    auto f16 = [&](const RConv &c) { return f16_mode && c.d_wt_f16 != nullptr && c.cin % 64 == 0 && c.cout % 64 == 0; };
+    // engine 3 (every convolution of stages 2-4), fp32 otherwise.  Which engine runs a convolution does not depend on its
+    // spatial dims, so this asks the kernel choice of the filter shape alone.
+    const int mode = iss_get_gemm_mode();
+    auto f16 = [&](const RConv &c) { return iss_conv_is_f16(iss_conv_kernel(conv_args(c), mode)); };
     auto conv = [&](const RConv &c, const float *in, bool in_packed, float *out, bool out_packed, int nb, int h, int w, int oh, int ow,
                     int flags, const float *residual, bool residual_packed) -> int {
-        ConvArgs a = {};
-        a.in = in; a.w = blob + c.w_off; a.pre_scale = blob + c.scale_off; a.pre_shift = blob + c.shift_off;
-        a.residual = residual; a.out = out;
-        if (c.d_wt) { a.wt_hi = c.d_wt; a.wt_lo = c.d_wt + (size_t)c.cout * c.Kp; a.wt_tiled = c.d_wt + 2 * (size_t)c.cout * c.Kp; a.Kp = c.Kp; }
-        a.wt_f16 = c.d_wt_f16; a.wt_f16_inv_scale = c.f16_inv_scale;
+        ConvArgs a = conv_args(c);
+        a.in = in; a.residual = residual; a.out = out;
         a.in_packed = in_packed; a.out_packed = out_packed; a.residual_packed = residual_packed;
-        a.M = (int64_t)nb * oh * ow; a.N = c.cout; a.K = c.kh * c.kw * c.cin;
-        a.H = h; a.W = w; a.C = c.cin; a.OH = oh; a.OW = ow;
-        a.KH = c.kh; a.KW = c.kw; a.SH = c.stride; a.SW = c.stride; a.PT = c.pad; a.PL = c.pad;
-        a.flags = ISS_F_AFFINE_PRE | flags | (residual ? ISS_F_RESIDUAL : 0);
-        return iss_launch_conv(a, false, st);
+        a.M = (int64_t)nb * oh * ow; a.H = h; a.W = w; a.OH = oh; a.OW = ow;
+        a.flags |= flags | (residual ? ISS_F_RESIDUAL : 0);
+        return iss_launch_conv(a, mode, st);
     };
 
     for (int w0 = 0; w0 < n_windows; w0 += (int)B) {
@@ -342,8 +333,8 @@ extern "C" int iss_resnet_embed(iss_ctx *ctx, iss_resnet *net, const float *d_fe
         a.M = nb; a.N = net->embed_dim; a.K = 2 * net->c_final * h;
         a.H = 1; a.W = 1; a.C = a.K; a.OH = 1; a.OW = 1; a.KH = 1; a.KW = 1; a.SH = 1; a.SW = 1;
         a.flags = ISS_F_BIAS;
-        if (net->d_emb_wt) { a.wt_hi = net->d_emb_wt; a.wt_lo = net->d_emb_wt + (size_t)net->embed_dim * net->emb_Kp; a.wt_tiled = net->d_emb_wt + 2 * (size_t)net->embed_dim * net->emb_Kp; a.Kp = net->emb_Kp; }
-        rc = iss_launch_conv(a, false, st);
+        a.wt = net->emb_wt;
+        rc = iss_launch_conv(a, mode, st);
         if (rc != ISS_OK) return rc;
     }
     return ISS_OK;
