@@ -17,6 +17,7 @@
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
+#include <type_traits>
 #include <vector>
 
 #include "conv_gemm.cuh"
@@ -41,6 +42,14 @@ struct Layer {
     int out_h, out_w, out_c;
     TcWeights wt;
 };
+
+// floating-point operations of one patch through the layer
+double layer_flops(const Layer &L)
+{
+    if (L.d.kind == ISS_LAYER_CONV2D) return 2.0 * L.out_h * L.out_w * (double)L.d.kh * L.d.kw * L.d.cin * L.d.cout;
+    if (L.d.kind == ISS_LAYER_DENSE) return 2.0 * (double)L.d.cin * L.d.cout;
+    return 0.0;
+}
 
 }  // namespace
 
@@ -113,102 +122,6 @@ patch_stats_kernel(const float *__restrict__ mspec, int ld, int w, int64_t n, Pa
     }
 }
 
-// ------------------------------------------------------------------ first layer: direct conv on the z-normalised patch
-// The first Conv2D has one input channel (K = kh*kw ~ 20), far too thin for a GEMM tile.  One CTA
-// stages a whole patch in shared memory, normalising each log-mel value exactly once with the
-// reference's arithmetic ((x - mean) / std in float32, segmenter.py:82), zero-padded for 'same'
-// convolutions; a thread owns 4 output channels x 4 consecutive output columns, so a filter tap is
-// one LDS.128 (weights) + 4 broadcast LDS.32 (inputs) for 16 FMAs.  Taps are accumulated in the
-// same (kh, kw) order as the implicit-GEMM kernel, so both produce identical bits.
-struct FirstArgs {
-    const float *mspec; int ld;
-    const int32_t *row0; const float *mu; const float *sigma;
-    const float *w, *bias, *pre_scale, *pre_shift, *post_scale, *post_shift;
-    float *out;
-    int64_t n;
-    int H, W, OH, OW, KH, KW, SH, SW, PT, PL, Hp, Wp, Cout, flags;
-    int out_packed;        // 1: store split-half words (lo16 << 16 | hi16) for the fp16-split convolution behind this layer
-};
-
-constexpr int FIRST_P = 4;
-
-__global__ void __launch_bounds__(256)
-conv_first_direct_kernel(const FirstArgs a)
-{
-    extern __shared__ __align__(16) float fsm[];
-    float *ws = fsm;                                   // [K][Cout]
-    float *xs = fsm + a.KH * a.KW * a.Cout;            // [Hp][Wp] (+ slack), zero border
-    const int tid = threadIdx.x;
-    const int CQ = a.Cout >> 2, streams = 256 / CQ;
-    const int c4 = tid % CQ, stream = tid / CQ;
-    const int K = a.KH * a.KW;
-    for (int i = tid; i < K * a.Cout; i += 256) ws[i] = a.w[i];
-    const int xs_len = a.Hp * a.Wp + FIRST_P * a.SW + a.KW;
-    float eb[4], es1[4], et1[4], es2[4], et2[4];
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-        const int c = c4 * 4 + q;
-        eb[q] = (a.flags & ISS_F_BIAS) ? a.bias[c] : 0.f;
-        es1[q] = (a.flags & ISS_F_AFFINE_PRE) ? a.pre_scale[c] : 1.f;  et1[q] = (a.flags & ISS_F_AFFINE_PRE) ? a.pre_shift[c] : 0.f;
-        es2[q] = (a.flags & ISS_F_AFFINE_POST) ? a.post_scale[c] : 1.f; et2[q] = (a.flags & ISS_F_AFFINE_POST) ? a.post_shift[c] : 0.f;
-    }
-    const int nblk = (a.OW + FIRST_P - 1) / FIRST_P;
-    const int G = a.OH * nblk;
-    for (int64_t img = blockIdx.x; img < a.n; img += gridDim.x) {
-        __syncthreads();                               // previous patch fully consumed (and ws visible)
-        for (int i = tid; i < xs_len; i += 256) xs[i] = 0.f;
-        __syncthreads();
-        const float mu = a.mu[img], sg = a.sigma[img];
-        const float *src = a.mspec + (int64_t)a.row0[img] * a.ld;
-        for (int e = tid; e < a.H * a.W; e += 256) {
-            const int r = e / a.W, c = e - r * a.W;
-            xs[(r + a.PT) * a.Wp + c + a.PL] = __fdiv_rn(__fsub_rn(__ldg(src + (int64_t)r * a.ld + c), mu), sg);
-        }
-        __syncthreads();
-        float *out_img = a.out + img * ((int64_t)a.OH * a.OW * a.Cout);
-        for (int g = stream; g < G; g += streams) {
-            const int oh = g / nblk, ow0 = (g - oh * nblk) * FIRST_P;
-            float acc[FIRST_P][4];
-#pragma unroll
-            for (int p = 0; p < FIRST_P; ++p)
-#pragma unroll
-                for (int q = 0; q < 4; ++q) acc[p][q] = 0.f;
-            for (int r = 0; r < a.KH; ++r) {
-                const float *xrow = xs + (oh * a.SH + r) * a.Wp + ow0 * a.SW;
-                const float *wrow = ws + (r * a.KW) * a.Cout + c4 * 4;
-                for (int t = 0; t < a.KW; ++t) {
-                    const float4 w4 = *reinterpret_cast<const float4 *>(wrow + t * a.Cout);
-#pragma unroll
-                    for (int p = 0; p < FIRST_P; ++p) {
-                        const float x = xrow[p * a.SW + t];
-                        acc[p][0] = fmaf(x, w4.x, acc[p][0]); acc[p][1] = fmaf(x, w4.y, acc[p][1]);
-                        acc[p][2] = fmaf(x, w4.z, acc[p][2]); acc[p][3] = fmaf(x, w4.w, acc[p][3]);
-                    }
-                }
-            }
-#pragma unroll
-            for (int p = 0; p < FIRST_P; ++p) {
-                if (ow0 + p >= a.OW) continue;
-                float y[4];
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    float v = acc[p][q] + eb[q];
-                    if (a.flags & ISS_F_AFFINE_PRE) v = fmaf(v, es1[q], et1[q]);
-                    if (a.flags & ISS_F_RELU) v = iss_relu(v);
-                    if (a.flags & ISS_F_SIGMOID) v = 1.f / (1.f + expf(-v));
-                    if (a.flags & ISS_F_AFFINE_POST) v = fmaf(v, es2[q], et2[q]);
-                    y[q] = v;
-                }
-                float *dst = out_img + ((int64_t)oh * a.OW + ow0 + p) * a.Cout + c4 * 4;
-                if (a.out_packed)
-                    *reinterpret_cast<uint4 *>(dst) = make_uint4(iss_pack_split(y[0]), iss_pack_split(y[1]), iss_pack_split(y[2]), iss_pack_split(y[3]));
-                else
-                    *reinterpret_cast<float4 *>(dst) = make_float4(y[0], y[1], y[2], y[3]);
-            }
-        }
-    }
-}
-
 // ------------------------------------------------------------------ first layer by linearity (FirstFuse, conv_gemm.cuh)
 // Y[r][x][c] = sum_{kh,kw} w[kh][kw][c] * mspec[f0 + r + kh][x + kw] in float64, for the frames a batch of patches
 // covers, stored as the two-float number Yh + Yl (FirstFuse, conv_gemm.cuh); one thread = one (row, column) position
@@ -268,92 +181,54 @@ first_coef_kernel(const float *__restrict__ mu, const float *__restrict__ sigma,
 }
 
 // ------------------------------------------------------------------ max pooling (NHWC)
+// One thread per lane T of the output, over [img][oh][ow][C / lane width]: one fp32 value (float), four fp32 values with
+// 16-byte loads and stores (float4, C % 4 == 0), or four split-half words (uint4, the tensor between two fp16-split
+// convolutions).  Words are compared on their decoded values hi + lo (exact in fp32) and the winning WORD is stored, so the value itself is
+// unchanged.  NaN propagates like TF's max; the first maximum wins.  The pooling layers are pure HBM traffic (218 KB in /
+// 53 KB out per patch for the first one).
+template <typename T>
 __global__ void __launch_bounds__(256)
-maxpool_nhwc_kernel(const float *__restrict__ in, float *__restrict__ out, int64_t total, int H, int W, int C,
+maxpool_nhwc_kernel(const T *__restrict__ in, T *__restrict__ out, int64_t total, int H, int W, int CL,
                     int OH, int OW, int KH, int KW, int SH, int SW, int PT, int PL)
 {
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;       // over [img][oh][ow][c]
+    constexpr int Q = sizeof(T) / sizeof(uint32_t);
+    constexpr bool WORDS = std::is_same<T, uint4>::value;
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= total) return;
-    const int c = (int)(i % C);
-    int64_t r = i / C;
+    const int c = (int)(i % CL);
+    int64_t r = i / CL;
     const int ow = (int)(r % OW); r /= OW;
     const int oh = (int)(r % OH);
     const int64_t img = r / OH;
-    float best = -INFINITY;
-    for (int y = 0; y < KH; ++y) {
-        const int ih = oh * SH - PT + y;
-        if (ih < 0 || ih >= H) continue;
-        for (int x = 0; x < KW; ++x) {
-            const int iw = ow * SW - PL + x;
-            if (iw < 0 || iw >= W) continue;
-            const float v = in[((img * H + ih) * W + iw) * C + c];
-            best = (v > best || v != v) ? v : best;        // NaN propagates like TF's max
-        }
-    }
-    out[i] = best;
-}
-
-// Four channels per thread (C % 4 == 0): 16-byte loads / stores, same window order and NaN rule as above.
-// The pooling layers are pure HBM traffic (218 KB in / 53 KB out per patch for the first one).
-__global__ void __launch_bounds__(256)
-maxpool_nhwc_vec4_kernel(const float4 *__restrict__ in, float4 *__restrict__ out, int64_t total4, int H, int W, int C4,
-                         int OH, int OW, int KH, int KW, int SH, int SW, int PT, int PL)
-{
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;       // over [img][oh][ow][c / 4]
-    if (i >= total4) return;
-    const int c = (int)(i % C4);
-    int64_t r = i / C4;
-    const int ow = (int)(r % OW); r /= OW;
-    const int oh = (int)(r % OH);
-    const int64_t img = r / OH;
-    float4 best = make_float4(-INFINITY, -INFINITY, -INFINITY, -INFINITY);
-    auto mx = [](float b, float v) { return (v > b || v != v) ? v : b; };
-    for (int y = 0; y < KH; ++y) {
-        const int ih = oh * SH - PT + y;
-        if (ih < 0 || ih >= H) continue;
-        for (int x = 0; x < KW; ++x) {
-            const int iw = ow * SW - PL + x;
-            if (iw < 0 || iw >= W) continue;
-            const float4 v = __ldg(in + ((img * H + ih) * W + iw) * C4 + c);
-            best.x = mx(best.x, v.x); best.y = mx(best.y, v.y); best.z = mx(best.z, v.z); best.w = mx(best.w, v.w);
-        }
-    }
-    out[i] = best;
-}
-
-// Pooling over split-half words (the tensor between two fp16-split convolutions): the window maximum is taken on
-// the decoded values hi + lo (exact in fp32) and the winning WORD is stored, so the value itself is unchanged.
-__global__ void __launch_bounds__(256)
-maxpool_nhwc_packed_kernel(const uint4 *__restrict__ in, uint4 *__restrict__ out, int64_t total4, int H, int W, int C4,
-                           int OH, int OW, int KH, int KW, int SH, int SW, int PT, int PL)
-{
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;       // over [img][oh][ow][c / 4]
-    if (i >= total4) return;
-    const int c = (int)(i % C4);
-    int64_t r = i / C4;
-    const int ow = (int)(r % OW); r /= OW;
-    const int oh = (int)(r % OH);
-    const int64_t img = r / OH;
-    float bv[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-    uint32_t bw[4];
+    float bv[Q];
+    uint32_t bw[Q];
 #pragma unroll
-    for (int q = 0; q < 4; ++q) bw[q] = iss_pack_split(-INFINITY);
+    for (int q = 0; q < Q; ++q) { bv[q] = -INFINITY; bw[q] = iss_pack_split(-INFINITY); }
     for (int y = 0; y < KH; ++y) {
         const int ih = oh * SH - PT + y;
         if (ih < 0 || ih >= H) continue;
         for (int x = 0; x < KW; ++x) {
             const int iw = ow * SW - PL + x;
             if (iw < 0 || iw >= W) continue;
-            const uint4 v = __ldg(in + ((img * H + ih) * W + iw) * C4 + c);
-            const uint32_t w4[4] = {v.x, v.y, v.z, v.w};
+            const T v = __ldg(in + ((img * H + ih) * W + iw) * CL + c);
+            const uint32_t *w = reinterpret_cast<const uint32_t *>(&v);
 #pragma unroll
-            for (int q = 0; q < 4; ++q) {
-                const float f = iss_unpack_split(w4[q]);
-                if (f > bv[q] || f != f) { bv[q] = f; bw[q] = w4[q]; }
+            for (int q = 0; q < Q; ++q) {
+                if constexpr (WORDS) {
+                    const float f = iss_unpack_split(w[q]);
+                    if (f > bv[q] || f != f) { bv[q] = f; bw[q] = w[q]; }
+                } else {
+                    const float f = __uint_as_float(w[q]);
+                    bv[q] = (f > bv[q] || f != f) ? f : bv[q];
+                }
             }
         }
     }
-    out[i] = make_uint4(bw[0], bw[1], bw[2], bw[3]);
+    T res;
+    uint32_t *rw = reinterpret_cast<uint32_t *>(&res);
+#pragma unroll
+    for (int q = 0; q < Q; ++q) rw[q] = WORDS ? bw[q] : __float_as_uint(bv[q]);
+    out[i] = res;
 }
 
 // ------------------------------------------------------------------ softmax head + non-finite override
@@ -412,14 +287,12 @@ extern "C" int iss_cnn_create(iss_ctx *ctx, const iss_layer_desc *layers, int n_
             if (d.kind == ISS_LAYER_CONV2D) {
                 ok = ok && d.cin == c && d.cout >= 1 && off_ok(d.w_off, (int64_t)d.kh * d.kw * d.cin * d.cout);
                 L.out_c = d.cout;
-                flops += 2.0 * L.out_h * L.out_w * (double)d.kh * d.kw * d.cin * d.cout;
             } else {
                 L.out_c = c;
             }
         } else if (d.kind == ISS_LAYER_DENSE) {
             ok = d.cin == h * w * c && d.cout >= 1 && off_ok(d.w_off, (int64_t)d.cin * d.cout);
             L.out_h = 1; L.out_w = 1; L.out_c = d.cout;
-            flops += 2.0 * (double)d.cin * d.cout;
         } else {
             ok = false;
         }
@@ -435,6 +308,7 @@ extern "C" int iss_cnn_create(iss_ctx *ctx, const iss_layer_desc *layers, int n_
             return ISS_ERR_UNSUPPORTED;
         }
         h = L.out_h; w = L.out_w; c = L.out_c;
+        flops += layer_flops(L);
         max_act = std::max<int64_t>(max_act, (int64_t)h * w * c);
         m->layers.push_back(L);
     }
@@ -515,18 +389,28 @@ extern "C" int64_t iss_cnn_workspace_bytes(const iss_cnn *cnn, int64_t n, int n_
 
 namespace {
 
+template <typename T>
+void launch_pool(const Layer &L, const float *in, float *out, int64_t nb, cudaStream_t st)
+{
+    constexpr int Q = sizeof(T) / sizeof(uint32_t);
+    const iss_layer_desc &d = L.d;
+    const int64_t total = nb * L.out_h * L.out_w * L.out_c / Q;
+    maxpool_nhwc_kernel<T><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(
+        reinterpret_cast<const T *>(in), reinterpret_cast<T *>(out), total, L.in_h, L.in_w, L.in_c / Q,
+        L.out_h, L.out_w, d.kh, d.kw, d.sh, d.sw, d.pad_top, d.pad_left);
+}
+
 // How iss_cnn_forward runs a layer
 enum class Step {
     FOLDED_POOL,        // 2x2 / stride-2 pooling taken in the next convolution's operand fill: nothing runs
-    POOL, POOL_VEC4, POOL_PACKED,   // maxpool_nhwc_kernel, maxpool_nhwc_vec4_kernel, maxpool_nhwc_packed_kernel
-    FIRST_DIRECT,       // conv_first_direct_kernel (unless the batch folds layer 0 into layer 1)
-    FIRST_GENERIC,      // the fp32 implicit GEMM gathering from the log-mel rows
-    CONV,               // iss_launch_conv
+    POOL,               // maxpool_nhwc_kernel
+    CONV,               // iss_launch_conv, unless the batch folds layer 0 into layer 1
 };
 
 struct LayerPlan {
     Step step;
-    // every step but the pooling ones: all but in, out, M, `first` and the patch arrays of the batch.  in_packed /
+    void (*pool)(const Layer &, const float *, float *, int64_t, cudaStream_t);     // POOL: launch_pool of the lane type
+    // CONV: all but in, out, M and `first` of the batch; layer 0 holds the log-mel source of the whole call.  in_packed /
     // out_packed are the activation formats, pool_h / pool_w the dims of a pooling folded into this layer.
     ConvArgs a;
 };
@@ -535,7 +419,8 @@ struct LayerPlan {
 // ISS_B200_FUSE_POOL / ISS_B200_FUSE_FIRST ("0": pooling / first layer as their own kernels) and the profiled layer,
 // all of which may change between calls.  *fuse_first: layer 0 may be folded into layer 1 (first_map: the workspace
 // holds the fused first layer's map and the ranges ascend), decided per batch by the frames its patches span.
-int plan_forward(const iss_cnn *cnn, int mode, bool first_map, std::vector<LayerPlan> &plan, bool *fuse_first)
+int plan_forward(const iss_cnn *cnn, int mode, const float *mspec, int ld, const PatchArrays &pa, bool first_map,
+                 std::vector<LayerPlan> &plan, bool *fuse_first)
 {
     const char *e = getenv("ISS_B200_FUSE_POOL");
     const bool fuse_pool = !(e && e[0] == '0');
@@ -566,6 +451,7 @@ int plan_forward(const iss_cnn *cnn, int mode, bool first_map, std::vector<Layer
             a.H = Lr.in_h; a.W = Lr.in_w; a.C = Lr.in_c; a.OH = Lr.out_h; a.OW = Lr.out_w;
             a.KH = d.kh; a.KW = d.kw; a.SH = d.sh; a.SW = d.sw; a.PT = d.pad_top; a.PL = d.pad_left;
         }
+        if (li == 0) { a.in = mspec; a.ld = ld; a.row0 = pa.row0; a.mu = pa.mu; a.sigma = pa.sigma; }
     }
     auto f16 = [&](const ConvArgs &a) { return iss_conv_is_f16(iss_conv_kernel(a, mode)); };
     // does compute layer j run on engine 3 when handed split-half words?
@@ -589,7 +475,8 @@ int plan_forward(const iss_cnn *cnn, int mode, bool first_map, std::vector<Layer
                 a.in_packed = 1; a.pool_h = Lr.in_h; a.pool_w = Lr.in_w;
                 if (f16(a)) { P.step = Step::FOLDED_POOL; pool_h = Lr.in_h; pool_w = Lr.in_w; continue; }
             }
-            P.step = packed ? Step::POOL_PACKED : (Lr.in_c % 4 == 0 ? Step::POOL_VEC4 : Step::POOL);
+            P.step = Step::POOL;
+            P.pool = packed ? launch_pool<uint4> : Lr.in_c % 4 == 0 ? launch_pool<float4> : launch_pool<float>;
             continue;
         }
         ConvArgs &a = P.a;
@@ -597,16 +484,15 @@ int plan_forward(const iss_cnn *cnn, int mode, bool first_map, std::vector<Layer
         a.pool_h = pool_h; a.pool_w = pool_w;
         pool_h = pool_w = 0;
         // split-half output iff the next compute layer reads it on engine 3; pooling layers in between keep the
-        // format (the packed pooling kernel moves 4 channels per thread)
+        // format (the word lane of the pooling kernel moves 4 channels per thread)
         size_t j = li + 1;
         bool pools_vec4 = true;
         for (; j < n && cnn->layers[j].d.kind == ISS_LAYER_MAXPOOL; ++j) pools_vec4 = pools_vec4 && cnn->layers[j].in_c % 4 == 0;
         const bool next_packed = j < n && pools_vec4 && reads_packed(j);
+        ISS_REQUIRE(li > 0 || d.kind == ISS_LAYER_CONV2D, ISS_ERR_UNSUPPORTED, "iss_cnn_forward: first layer must be Conv2D");
+        P.step = Step::CONV;
+        a.out_packed = next_packed && iss_conv_writes_words(iss_conv_kernel(a, mode));
         if (li == 0) {
-            ISS_REQUIRE(d.kind == ISS_LAYER_CONV2D, ISS_ERR_UNSUPPORTED, "iss_cnn_forward: first layer must be Conv2D");
-            const bool direct = d.cin == 1 && (d.cout == 16 || d.cout == 32 || d.cout == 64 || d.cout == 128) && !(d.flags & ISS_F_SOFTMAX);
-            P.step = direct ? Step::FIRST_DIRECT : Step::FIRST_GENERIC;
-            a.out_packed = direct && next_packed;            // the generic first layer writes fp32
             // the fused first layer (FirstFuse, conv_gemm.cuh): the direct kernel's shape without padding / stride, in
             // layer 1's slab-kernel operand fill
             *fuse_first = false;
@@ -618,9 +504,6 @@ int plan_forward(const iss_cnn *cnn, int mode, bool first_map, std::vector<Layer
                 a1.in_packed = 1; a1.first = &probe;
                 *fuse_first = f16(a1);
             }
-        } else {
-            P.step = Step::CONV;
-            a.out_packed = next_packed && f16(a);
         }
         packed = a.out_packed;
     }
@@ -693,7 +576,7 @@ extern "C" int iss_cnn_forward(iss_ctx *ctx, iss_cnn *cnn, const float *d_mspec,
     const int mode = iss_get_gemm_mode();
     std::vector<LayerPlan> plan;
     bool fuse_first = false;
-    const int prc = plan_forward(cnn, mode, d_first_yh && ranges_ascending, plan, &fuse_first);
+    const int prc = plan_forward(cnn, mode, d_mspec, ld, pa, d_first_yh && ranges_ascending, plan, &fuse_first);
     if (prc != ISS_OK) return prc;
     ISS_CUDA_OK(cudaMemcpyAsync(d_seg_start, h_seg_start, sizeof(int32_t) * n_seg, cudaMemcpyHostToDevice, st));
     ISS_CUDA_OK(cudaMemcpyAsync(d_seg_off, off.data(), sizeof(int64_t) * (n_seg + 1), cudaMemcpyHostToDevice, st));
@@ -728,26 +611,16 @@ extern "C" int iss_cnn_forward(iss_ctx *ctx, iss_cnn *cnn, const float *d_mspec,
                 }
                 ISS_CUDA_OK(cudaEventRecord(cnn->prof_ev[cnn->prof_used], st));
             }
-            if (P.step == Step::POOL || P.step == Step::POOL_VEC4 || P.step == Step::POOL_PACKED) {
-                const int64_t total = nb * Lr.out_h * Lr.out_w * Lr.out_c;
-                if (P.step == Step::POOL_PACKED)
-                    maxpool_nhwc_packed_kernel<<<(unsigned)((total / 4 + 255) / 256), 256, 0, st>>>(
-                        reinterpret_cast<const uint4 *>(cur), reinterpret_cast<uint4 *>(dst), total / 4, Lr.in_h, Lr.in_w, Lr.in_c / 4,
-                        Lr.out_h, Lr.out_w, d.kh, d.kw, d.sh, d.sw, d.pad_top, d.pad_left);
-                else if (P.step == Step::POOL_VEC4)
-                    maxpool_nhwc_vec4_kernel<<<(unsigned)((total / 4 + 255) / 256), 256, 0, st>>>(
-                        reinterpret_cast<const float4 *>(cur), reinterpret_cast<float4 *>(dst), total / 4, Lr.in_h, Lr.in_w, Lr.in_c / 4,
-                        Lr.out_h, Lr.out_w, d.kh, d.kw, d.sh, d.sw, d.pad_top, d.pad_left);
-                else
-                    maxpool_nhwc_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(cur, dst, total, Lr.in_h, Lr.in_w, Lr.in_c,
-                        Lr.out_h, Lr.out_w, d.kh, d.kw, d.sh, d.sw, d.pad_top, d.pad_left);
+            if (P.step == Step::POOL) {
+                P.pool(Lr, cur, dst, nb, st);
                 ISS_CUDA_OK(cudaGetLastError());
                 iss_count_launch();
             } else {
                 ConvArgs a = P.a;
                 a.out = dst;
                 a.M = nb * a.OH * a.OW;
-                int rc = ISS_OK;
+                if (a.row0) { a.row0 += b0; a.mu += b0; a.sigma += b0; }
+                else a.in = cur;
                 if (li == 0 && fuse_first) {
                     // the float64 map of the first layer covers the frames this batch's patches span, if few enough
                     const int64_t f_first = host_row0(b0), f_last = host_row0(b0 + nb - 1);
@@ -757,46 +630,25 @@ extern "C" int iss_cnn_forward(iss_ctx *ctx, iss_cnn *cnn, const float *d_mspec,
                         first_linear_kernel<<<(unsigned)((work + 255) / 256), 256, (size_t)d.kh * d.kw * d.cout * sizeof(float), st>>>(
                             d_mspec, ld, f_first, rows, L, Lr.out_w, d.kh, d.kw, d.cout, a.w, d_first_yh, d_first_yl);
                         first_coef_kernel<<<(unsigned)((nb * d.cout + 255) / 256), 256, 0, st>>>(
-                            pa.mu + b0, pa.sigma + b0, cnn->d_first_S, a.bias, a.pre_scale, a.pre_shift, nb, d.cout, d_first_coef);
+                            a.mu, a.sigma, cnn->d_first_S, a.bias, a.pre_scale, a.pre_shift, nb, d.cout, d_first_coef);
                         ISS_CUDA_OK(cudaGetLastError());
                         iss_count_launch(2);
                         ffuse.Yh = d_first_yh; ffuse.Yl = d_first_yl; ffuse.y_f0 = f_first; ffuse.y_rows = rows;
-                        ffuse.row0 = pa.row0 + b0; ffuse.coef = d_first_coef;
+                        ffuse.row0 = a.row0; ffuse.coef = d_first_coef;
                         ffuse.post_scale = a.post_scale; ffuse.post_shift = a.post_shift; ffuse.flags = a.flags; ffuse.n_img = nb;
                         first_fused = true;                      // nothing stored: layer 1 reads the map
                     }
                 }
-                if (P.step == Step::FIRST_DIRECT && !first_fused) {
-                    FirstArgs f = {};
-                    f.mspec = d_mspec; f.ld = ld; f.row0 = pa.row0 + b0; f.mu = pa.mu + b0; f.sigma = pa.sigma + b0;
-                    f.w = a.w; f.bias = a.bias; f.pre_scale = a.pre_scale; f.pre_shift = a.pre_shift;
-                    f.post_scale = a.post_scale; f.post_shift = a.post_shift; f.out = dst; f.n = nb;
-                    f.H = Lr.in_h; f.W = Lr.in_w; f.OH = Lr.out_h; f.OW = Lr.out_w; f.KH = d.kh; f.KW = d.kw;
-                    f.SH = d.sh; f.SW = d.sw; f.PT = d.pad_top; f.PL = d.pad_left;
-                    f.Hp = Lr.in_h + d.pad_top + d.pad_bottom; f.Wp = Lr.in_w + d.pad_left + d.pad_right;
-                    f.Cout = d.cout; f.flags = a.flags; f.out_packed = a.out_packed;
-                    const size_t smem = ((size_t)d.kh * d.kw * d.cout + (size_t)f.Hp * f.Wp + FIRST_P * d.sw + d.kw + 8) * sizeof(float);
-                    ISS_REQUIRE(smem <= 200 * 1024, ISS_ERR_UNSUPPORTED, "iss_cnn_forward: first layer too large for the first-layer kernel");
-                    ISS_CUDA_OK(iss_optin_smem(reinterpret_cast<const void *>(conv_first_direct_kernel), 200 * 1024));
-                    const unsigned grid = (unsigned)std::min<int64_t>(nb, (int64_t)ctx->sm_count * 8);
-                    conv_first_direct_kernel<<<grid, 256, smem, st>>>(f);
-                    ISS_CUDA_OK(cudaGetLastError());
-                    iss_count_launch();
-                } else if (P.step == Step::FIRST_GENERIC) {
-                    a.in = d_mspec; a.ld = ld; a.row0 = pa.row0 + b0; a.mu = pa.mu + b0; a.sigma = pa.sigma + b0;
-                    rc = iss_launch_conv(a, mode, st);
-                } else if (P.step == Step::CONV) {
-                    a.in = cur;
-                    if (li == 1 && first_fused) { a.first = &ffuse; a.in = nullptr; }
-                    rc = iss_launch_conv(a, mode, st);
+                if (li == 1 && first_fused) { a.first = &ffuse; a.in = nullptr; }
+                if (!(li == 0 && first_fused)) {
+                    const int rc = iss_launch_conv(a, mode, st);
+                    if (rc != ISS_OK) return rc;
                 }
-                if (rc != ISS_OK) return rc;
             }
             if (prof) {
                 ISS_CUDA_OK(cudaEventRecord(cnn->prof_ev[cnn->prof_used + 1], st));
                 cnn->prof_used += 2;
-                if (d.kind == ISS_LAYER_CONV2D) cnn->prof_flops += 2.0 * nb * Lr.out_h * Lr.out_w * (double)d.kh * d.kw * d.cin * d.cout;
-                else if (d.kind == ISS_LAYER_DENSE) cnn->prof_flops += 2.0 * nb * (double)d.cin * d.cout;
+                cnn->prof_flops += nb * layer_flops(Lr);
             }
             cur = dst;
             which ^= 1;
@@ -841,8 +693,5 @@ extern "C" int iss_cnn_num_layers(const iss_cnn *cnn) { return cnn ? (int)cnn->l
 extern "C" double iss_cnn_layer_flops(const iss_cnn *cnn, int layer)
 {
     if (!cnn || layer < 0 || layer >= (int)cnn->layers.size()) return 0.0;
-    const Layer &L = cnn->layers[layer];
-    if (L.d.kind == ISS_LAYER_CONV2D) return 2.0 * L.out_h * L.out_w * (double)L.d.kh * L.d.kw * L.d.cin * L.d.cout;
-    if (L.d.kind == ISS_LAYER_DENSE) return 2.0 * (double)L.d.cin * L.d.cout;
-    return 0.0;
+    return layer_flops(cnn->layers[layer]);
 }

@@ -134,17 +134,12 @@ conv_gemm_f32_kernel(const ConvArgs a)
         __syncthreads();
     }
 
-    // ---- epilogue: bias -> affine(pre) -> relu -> affine(post) ----
-    float eb[TN], es1[TN], et1[TN], es2[TN], et2[TN];
+    // ---- epilogue ----
+    EpiCoef1 cf[TN];
 #pragma unroll
     for (int j = 0; j < TN; ++j) {
         const int n = n0 + tx * TN + j;
-        const bool ok = n < a.N;
-        eb[j] = (ok && (a.flags & ISS_F_BIAS)) ? a.bias[n] : 0.f;
-        es1[j] = (ok && (a.flags & ISS_F_AFFINE_PRE)) ? a.pre_scale[n] : 1.f;
-        et1[j] = (ok && (a.flags & ISS_F_AFFINE_PRE)) ? a.pre_shift[n] : 0.f;
-        es2[j] = (ok && (a.flags & ISS_F_AFFINE_POST)) ? a.post_scale[n] : 1.f;
-        et2[j] = (ok && (a.flags & ISS_F_AFFINE_POST)) ? a.post_shift[n] : 0.f;
+        if (n < a.N) cf[j] = epi_coef1(a, n);
     }
 #pragma unroll
     for (int i = 0; i < TM; ++i) {
@@ -153,13 +148,9 @@ conv_gemm_f32_kernel(const ConvArgs a)
         float v[TN];
 #pragma unroll
         for (int j = 0; j < TN; ++j) {
-            float x = acc[i][j] + eb[j];
-            if (a.flags & ISS_F_AFFINE_PRE) x = fmaf(x, es1[j], et1[j]);
-            if (a.flags & ISS_F_RESIDUAL) { const int n = n0 + tx * TN + j; if (n < a.N) x += __ldg(a.residual + mr * a.N + n); }
-            if (a.flags & ISS_F_RELU) x = iss_relu(x);
-            if (a.flags & ISS_F_SIGMOID) x = 1.f / (1.f + expf(-x));
-            if (a.flags & ISS_F_AFFINE_POST) x = fmaf(x, es2[j], et2[j]);
-            v[j] = x;
+            const int n = n0 + tx * TN + j;
+            const float r = (a.flags & ISS_F_RESIDUAL) && n < a.N ? __ldg(a.residual + mr * a.N + n) : 0.f;
+            v[j] = epi_f32<true>(cf[j], a.flags, acc[i][j], r);
         }
         float *o = a.out + mr * a.N + n0 + tx * TN;
         if (vecB && n0 + tx * TN + TN <= a.N) {
@@ -210,15 +201,104 @@ dense_small_n_kernel(const ConvArgs a)
             float xv = 0.f;
 #pragma unroll
             for (int n = 0; n < SMALL_N; ++n) if (n == lane) xv = acc[n];
-            const int n = lane;
-            if (a.flags & ISS_F_BIAS) xv += a.bias[n];
-            if (a.flags & ISS_F_AFFINE_PRE) xv = fmaf(xv, a.pre_scale[n], a.pre_shift[n]);
-            if (a.flags & ISS_F_RELU) xv = iss_relu(xv);
-            if (a.flags & ISS_F_SIGMOID) xv = 1.f / (1.f + expf(-xv));
-            if (a.flags & ISS_F_AFFINE_POST) xv = fmaf(xv, a.post_scale[n], a.post_shift[n]);
-            a.out[m * a.N + n] = xv;
+            a.out[m * a.N + lane] = epi_f32(epi_coef1(a, lane), a.flags, xv);
         }
     }
+}
+
+// ------------------------------------------------------------------ first layer: direct conv on the z-normalised patch
+// The first Conv2D has one input channel (K = kh*kw ~ 20), far too thin for a GEMM tile.  One CTA
+// stages a whole patch in shared memory, normalising each log-mel value exactly once with the
+// reference's arithmetic ((x - mean) / std in float32, segmenter.py:82), zero-padded for 'same'
+// convolutions; a thread owns 4 output channels x 4 consecutive output columns, so a filter tap is
+// one LDS.128 (weights) + 4 broadcast LDS.32 (inputs) for 16 FMAs.  Taps are accumulated in the
+// same (kh, kw) order as the implicit-GEMM kernel, so both produce identical bits.
+constexpr int FIRST_P = 4;
+
+// the zero-padded patch: H + PT + PB rows by W + PL + PR columns, for 'valid' and Keras 'same' padding alike
+__host__ __device__ inline int first_hp(const ConvArgs &a) { return max(a.H + a.PT, (a.OH - 1) * a.SH + a.KH); }
+__host__ __device__ inline int first_wp(const ConvArgs &a) { return max(a.W + a.PL, (a.OW - 1) * a.SW + a.KW); }
+
+__global__ void __launch_bounds__(256)
+conv_first_direct_kernel(const ConvArgs a)
+{
+    extern __shared__ __align__(16) float fsm[];
+    const int Cout = a.N, Hp = first_hp(a), Wp = first_wp(a);
+    float *ws = fsm;                                   // [K][Cout]
+    float *xs = fsm + a.KH * a.KW * Cout;              // [Hp][Wp] (+ slack), zero border
+    const int tid = threadIdx.x;
+    const int CQ = Cout >> 2, streams = 256 / CQ;
+    const int c4 = tid % CQ, stream = tid / CQ;
+    const int K = a.KH * a.KW;
+    for (int i = tid; i < K * Cout; i += 256) ws[i] = a.w[i];
+    const int xs_len = Hp * Wp + FIRST_P * a.SW + a.KW;
+    EpiCoef1 cf[4];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) cf[q] = epi_coef1(a, c4 * 4 + q);
+    const int nblk = (a.OW + FIRST_P - 1) / FIRST_P;
+    const int G = a.OH * nblk;
+    const int64_t ohw = (int64_t)a.OH * a.OW;
+    for (int64_t img = blockIdx.x; img * ohw < a.M; img += gridDim.x) {       // M / ohw patches
+        __syncthreads();                               // previous patch fully consumed (and ws visible)
+        for (int i = tid; i < xs_len; i += 256) xs[i] = 0.f;
+        __syncthreads();
+        const float mu = a.mu[img], sg = a.sigma[img];
+        const float *src = a.in + (int64_t)a.row0[img] * a.ld;
+        for (int e = tid; e < a.H * a.W; e += 256) {
+            const int r = e / a.W, c = e - r * a.W;
+            xs[(r + a.PT) * Wp + c + a.PL] = __fdiv_rn(__fsub_rn(__ldg(src + (int64_t)r * a.ld + c), mu), sg);
+        }
+        __syncthreads();
+        float *out_img = a.out + img * ohw * Cout;
+        for (int g = stream; g < G; g += streams) {
+            const int oh = g / nblk, ow0 = (g - oh * nblk) * FIRST_P;
+            float acc[FIRST_P][4];
+#pragma unroll
+            for (int p = 0; p < FIRST_P; ++p)
+#pragma unroll
+                for (int q = 0; q < 4; ++q) acc[p][q] = 0.f;
+            for (int r = 0; r < a.KH; ++r) {
+                const float *xrow = xs + (oh * a.SH + r) * Wp + ow0 * a.SW;
+                const float *wrow = ws + (r * a.KW) * Cout + c4 * 4;
+                for (int t = 0; t < a.KW; ++t) {
+                    const float4 w4 = *reinterpret_cast<const float4 *>(wrow + t * Cout);
+#pragma unroll
+                    for (int p = 0; p < FIRST_P; ++p) {
+                        const float x = xrow[p * a.SW + t];
+                        acc[p][0] = fmaf(x, w4.x, acc[p][0]); acc[p][1] = fmaf(x, w4.y, acc[p][1]);
+                        acc[p][2] = fmaf(x, w4.z, acc[p][2]); acc[p][3] = fmaf(x, w4.w, acc[p][3]);
+                    }
+                }
+            }
+#pragma unroll
+            for (int p = 0; p < FIRST_P; ++p) {
+                if (ow0 + p >= a.OW) continue;
+                float y[4];
+#pragma unroll
+                for (int q = 0; q < 4; ++q) y[q] = epi_f32(cf[q], a.flags, acc[p][q]);
+                float *dst = out_img + ((int64_t)oh * a.OW + ow0 + p) * Cout + c4 * 4;
+                if (a.out_packed)
+                    *reinterpret_cast<uint4 *>(dst) = make_uint4(iss_pack_split(y[0]), iss_pack_split(y[1]), iss_pack_split(y[2]), iss_pack_split(y[3]));
+                else
+                    *reinterpret_cast<float4 *>(dst) = make_float4(y[0], y[1], y[2], y[3]);
+            }
+        }
+    }
+}
+
+int launch_first_direct(const ConvArgs &a, cudaStream_t st)
+{
+    const size_t smem = ((size_t)a.KH * a.KW * a.N + (size_t)first_hp(a) * first_wp(a) + FIRST_P * a.SW + a.KW + 8) * sizeof(float);
+    ISS_REQUIRE(smem <= 200 * 1024, ISS_ERR_UNSUPPORTED, "conv: first layer too large for the first-layer kernel");
+    ISS_CUDA_OK(iss_optin_smem(reinterpret_cast<const void *>(conv_first_direct_kernel), 200 * 1024));
+    int dev = 0, sms = 0;
+    ISS_CUDA_OK(cudaGetDevice(&dev));
+    ISS_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    const int64_t n_img = a.M / ((int64_t)a.OH * a.OW);
+    conv_first_direct_kernel<<<(unsigned)std::min<int64_t>(n_img, (int64_t)sms * 8), 256, smem, st>>>(a);
+    ISS_CUDA_OK(cudaGetLastError());
+    iss_count_launch();
+    return ISS_OK;
 }
 
 bool small_n_covers(const ConvArgs &a)
@@ -248,10 +328,11 @@ int launch_conv_t(const ConvArgs &a, cudaStream_t st)
 
 IssConvKernel iss_conv_kernel(const ConvArgs &a, int mode)
 {
-    if (a.row0) return ISS_CONV_F32_FIRST;
+    if (a.row0)
+        return a.C == 1 && (a.N == 16 || a.N == 32 || a.N == 64 || a.N == 128) ? ISS_CONV_FIRST_DIRECT : ISS_CONV_F32_FIRST;
     if (small_n_covers(a)) return ISS_CONV_SMALL_N;
-    if (mode == ISS_GEMM_FP32 || !a.wt.tiled) return ISS_CONV_F32;
-    if (mode == ISS_GEMM_TC_F16 && a.wt.f16 && !(a.flags & ISS_F_SIGMOID)) {
+    if (mode == ISS_GEMM_FP32 || !a.wt.tiled || (a.flags & ISS_F_SIGMOID)) return ISS_CONV_F32;
+    if (mode == ISS_GEMM_TC_F16 && a.wt.f16) {
         const bool slab = iss_slab_covers(a);
         // folded pooling: 2x2 / stride-2 'valid' over split-half words, in the gather kernel's operand fill
         const bool pool_ok = a.pool_h == 0 || (!a.first && a.in_packed && a.pool_h / 2 == a.H && a.pool_w / 2 == a.W);
@@ -265,10 +346,12 @@ IssConvKernel iss_conv_kernel(const ConvArgs &a, int mode)
 int iss_launch_conv(const ConvArgs &a, int mode, cudaStream_t st)
 {
     const IssConvKernel k = iss_conv_kernel(a, mode);
-    ISS_REQUIRE(iss_conv_is_f16(k) || (!a.in_packed && !a.out_packed && !a.residual_packed && !a.first && a.pool_h == 0), ISS_ERR_UNSUPPORTED,
+    ISS_REQUIRE((iss_conv_is_f16(k) || (!a.in_packed && !a.residual_packed && !a.first && a.pool_h == 0)) &&
+                (iss_conv_writes_words(k) || !a.out_packed), ISS_ERR_UNSUPPORTED,
                 "conv: split-half tensors, folded pooling and the fused first layer need the fp16-split engine");
     switch (k) {
     case ISS_CONV_F32_FIRST: return launch_conv_t<true>(a, st);
+    case ISS_CONV_FIRST_DIRECT: return launch_first_direct(a, st);
     case ISS_CONV_SMALL_N: {
         const int64_t gm = (a.M + 7) / 8;
         dense_small_n_kernel<<<(unsigned)(gm < 132 * 8 ? gm : 132 * 8), 256, (size_t)a.K * a.N * sizeof(float), st>>>(a);

@@ -95,6 +95,35 @@ struct ConvArgs {
     const FirstFuse *first;         // host pointer, non-null: the fused first layer (copied into the kernel parameters)
 };
 
+// Epilogue coefficients of output channel n: bias, pre-affine (s1, t1), post-affine (s2, t2); absent terms are identities.
+struct EpiCoef1 {
+    float eb = 0.f, es1 = 1.f, et1 = 0.f, es2 = 1.f, et2 = 0.f;
+};
+
+__device__ __forceinline__ EpiCoef1 epi_coef1(const ConvArgs &a, int n)
+{
+    const bool pre = a.flags & ISS_F_AFFINE_PRE, post = a.flags & ISS_F_AFFINE_POST;
+    EpiCoef1 c;
+    c.eb = (a.flags & ISS_F_BIAS) ? __ldg(a.bias + n) : 0.f;
+    c.es1 = pre ? __ldg(a.pre_scale + n) : 1.f;  c.et1 = pre ? __ldg(a.pre_shift + n) : 0.f;
+    c.es2 = post ? __ldg(a.post_scale + n) : 1.f; c.et2 = post ? __ldg(a.post_shift + n) : 0.f;
+    return c;
+}
+
+// The epilogue of the fp32 kernels: bias -> pre-affine -> (+ residual r) -> ReLU -> sigmoid -> post-affine.  Kernels that
+// never take a residual (RESID = false) leave its test out, which keeps their register count.
+template <bool RESID = false>
+__device__ __forceinline__ float epi_f32(const EpiCoef1 &c, int flags, float acc, float r = 0.f)
+{
+    float v = acc + c.eb;
+    if (flags & ISS_F_AFFINE_PRE) v = fmaf(v, c.es1, c.et1);
+    if (RESID && (flags & ISS_F_RESIDUAL)) v += r;
+    if (flags & ISS_F_RELU) v = iss_relu(v);
+    if (flags & ISS_F_SIGMOID) v = 1.f / (1.f + expf(-v));
+    if (flags & ISS_F_AFFINE_POST) v = fmaf(v, c.es2, c.et2);
+    return v;
+}
+
 #define ISS_GEMM_FP32  0      /* fp32 CUDA cores (conv_gemm.cu) */
 #define ISS_GEMM_TC_TS 2      /* wgmma 3xTF32 (conv_gemm_tc.cu): every layer shape with C, K, N multiples of 32 */
 #define ISS_GEMM_TC_F16 3     /* wgmma fp16 hi/lo split (conv_gemm_tc.cu) for layers with C, N multiples of 64; other layers as engine 2 */
@@ -110,17 +139,20 @@ extern "C" int iss_get_gemm_mode(void);
 int iss_prepare_weights(const float *h_w, int C, int K, int N, bool f16, TcWeights *w);
 void iss_free_weights(TcWeights *w);
 
-// The kernel that runs a layer.  Only the engine-3 kernels (iss_conv_is_f16) read or write split-half words, take a
-// folded pooling (pool_h > 0) or the fused first layer (`first`).
+// The kernel that runs a layer.  Only the engine-3 kernels (iss_conv_is_f16) read split-half words, take a folded
+// pooling (pool_h > 0) or the fused first layer (`first`); they and the direct first-layer kernel write them
+// (iss_conv_writes_words).  Layers with a sigmoid run on the fp32 kernels, the only ones that evaluate it.
 enum IssConvKernel {
     ISS_CONV_F32,           // fp32 CUDA cores (conv_gemm.cu)
     ISS_CONV_F32_FIRST,     // the same, gathering the generic first layer's patches from the log-mel rows
+    ISS_CONV_FIRST_DIRECT,  // first layer with one input channel and 16, 32, 64 or 128 outputs, one patch per CTA
     ISS_CONV_SMALL_N,       // fp32 dense / 1x1 layer with at most 8 outputs (the softmax heads)
     ISS_CONV_TF32,          // engine 2, gather kernel
     ISS_CONV_F16,           // engine 3, gather kernel
     ISS_CONV_F16_SLAB,      // engine 3, slab kernel
 };
 inline bool iss_conv_is_f16(IssConvKernel k) { return k == ISS_CONV_F16 || k == ISS_CONV_F16_SLAB; }
+inline bool iss_conv_writes_words(IssConvKernel k) { return iss_conv_is_f16(k) || k == ISS_CONV_FIRST_DIRECT; }
 IssConvKernel iss_conv_kernel(const ConvArgs &a, int mode);
 
 // the tensor-core launchers behind iss_launch_conv (conv_gemm_tc.cu)

@@ -134,21 +134,8 @@ __device__ __forceinline__ void epi_store(const ConvArgs &a, const EpiCoef &c, i
     else *reinterpret_cast<float2 *>(dst) = make_float2(y[0], y[1]);
 }
 
-// The same epilogue for the single engine-3 output (m, n) (the slab kernel, whose accumulator rows are channels).
-struct EpiCoef1 {
-    float eb, es1, et1, es2, et2;
-};
-
-__device__ __forceinline__ EpiCoef1 epi_coef1(const ConvArgs &a, int n)
-{
-    const bool pre = a.flags & ISS_F_AFFINE_PRE, post = a.flags & ISS_F_AFFINE_POST;
-    EpiCoef1 c;
-    c.eb = (a.flags & ISS_F_BIAS) ? __ldg(a.bias + n) : 0.f;
-    c.es1 = pre ? __ldg(a.pre_scale + n) : 1.f;  c.et1 = pre ? __ldg(a.pre_shift + n) : 0.f;
-    c.es2 = post ? __ldg(a.post_scale + n) : 1.f; c.et2 = post ? __ldg(a.post_shift + n) : 0.f;
-    return c;
-}
-
+// The same epilogue for the single engine-3 output (m, n) (the slab kernel, whose accumulator rows are channels), with
+// the coefficients of epi_coef1 (conv_gemm.cuh).
 __device__ __forceinline__ void epi_store1(const ConvArgs &a, const EpiCoef1 &c, int64_t m, int n, float y, float inv_scale)
 {
     float v = fmaf(y, inv_scale * c.es1, fmaf(c.eb, c.es1, c.et1));
@@ -267,7 +254,7 @@ conv_gemm_wg_kernel(const ConvArgs a, const unsigned char *__restrict__ wt, floa
             } else {
                 static_assert(MODE == LD_POOL, "the fused first layer runs in conv_slab_kernel");
                 // the 2x2 window of the un-pooled NHWC tensor [img][pool_h][pool_w][C]: the WORD of the largest value is kept
-                // (as maxpool_nhwc_packed_kernel does: window order (0,0) (0,1) (1,0) (1,1), NaN wins, first maximum wins)
+                // (as maxpool_nhwc_kernel<uint4> does: window order (0,0) (0,1) (1,0) (1,1), NaN wins, first maximum wins)
                 uint32_t bw[8] = {0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
                 int ih, iw;
                 if (pixel_ok(i, ih, iw)) {

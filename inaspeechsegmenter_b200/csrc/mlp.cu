@@ -84,7 +84,7 @@ extern "C" int iss_mlp_forward(iss_ctx *ctx, iss_mlp *m, const float *d_x, int64
         a.out = (i + 1 == m->layers.size()) ? d_y : buf[i & 1];
         a.M = n_rows; a.N = d.cout; a.K = d.cin; a.H = 1; a.W = 1; a.C = d.cin; a.OH = 1; a.OW = 1;
         a.KH = 1; a.KW = 1; a.SH = 1; a.SW = 1; a.flags = d.flags;
-        int rc = iss_launch_conv(a, false, st);       // no tensor-core weights prepared => fp32 kernel
+        int rc = iss_launch_conv(a, ISS_GEMM_FP32, st);
         if (rc != ISS_OK) return rc;
         cur = a.out;
     }

@@ -103,8 +103,8 @@ def _engine_u(d, li, in_shape, mode):
     """Unit error of the engine a layer runs on (the dispatch of cnn.cu / conv_gemm.cu, by shape)."""
     if li == 0:
         return U_FIRST
-    if d['kind'] == LAYER_MAXPOOL or mode == 0:
-        return U32
+    if d['kind'] == LAYER_MAXPOOL or mode == 0 or d['flags'] & F_SIGMOID:
+        return U32                                     # only the fp32 kernels evaluate a sigmoid
     cin = d['cin']
     K = cin if d['kind'] == LAYER_DENSE else d['kh'] * d['kw'] * cin
     N = d['cout']

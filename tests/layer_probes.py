@@ -47,7 +47,7 @@ class ProbeNet:
             self.bn(ch)
 
     def conv(self, cout, k=(3, 3), s=(1, 1), padding='valid', bias=True, pre=False, relu=False, post=False, gain=1.0,
-             kernel=None):
+             kernel=None, act='linear'):
         h, w, cin = self.shape
         name = self._name('conv')
         if kernel is None:
@@ -57,7 +57,7 @@ class ProbeNet:
             self.weights[name + '/bias'] = self.rng.normal(0, 0.05, cout).astype(np.float32)
         self.layers.append({'class_name': 'Conv2D', 'config': {
             'name': name, 'filters': cout, 'kernel_size': list(k), 'strides': list(s), 'padding': padding,
-            'use_bias': bias, 'activation': 'linear'}})
+            'use_bias': bias, 'activation': act}})
         self._epilogue(cout, pre, relu, post)
         self.shape = (_out(h, k[0], s[0], padding), _out(w, k[1], s[1], padding), cout)
         return self
@@ -84,7 +84,7 @@ class ProbeNet:
         self.shape = (_out(h, p[0], s[0], padding), _out(w, p[1], s[1], padding), c)
         return self
 
-    def dense(self, units, pre=False, relu=False, post=False):
+    def dense(self, units, pre=False, relu=False, post=False, act='linear'):
         if len(self.shape) == 3:
             self.layers.append({'class_name': 'Flatten', 'config': {'name': self._name('flat')}})
         cin = int(np.prod(self.shape))
@@ -92,7 +92,7 @@ class ProbeNet:
         self.weights[name + '/kernel'] = (self.rng.standard_normal((cin, units)) * np.sqrt(2.0 / cin)).astype(np.float32)
         self.weights[name + '/bias'] = self.rng.normal(0, 0.05, units).astype(np.float32)
         self.layers.append({'class_name': 'Dense', 'config': {'name': name, 'units': units, 'use_bias': True,
-                                                              'activation': 'linear'}})
+                                                              'activation': act}})
         self._epilogue(units, pre, relu, post)
         self.shape = (units,)
         return self
@@ -252,7 +252,18 @@ def _cases():
     # ---- max-pooling on split-half words, 'same' padding (-inf words at the border)
     c['pool_words_3x2_same'] = lambda: dict(
         net=_first(21).conv(64, (3, 3), pre=True, relu=True).pool((3, 2), (2, 2), 'same').conv(64, (3, 3), padding='same', pre=True, relu=True),
-        kernels=['maxpool_nhwc_packed_kernel', 'conv_gemm_wg_kernel<1,64,1>'])
+        kernels=['maxpool_nhwc_kernel<uint4>', 'conv_gemm_wg_kernel<1,64,1>'])
+    # ---- max-pooling on fp32 values: four channels per thread ('same' padding, engine 2), and one (6 channels)
+    c['pool_f32x4_3x2_same_mode2'] = lambda: dict(
+        net=_first(21).conv(64, (3, 3), pre=True, relu=True).pool((3, 2), (2, 2), 'same').conv(64, (3, 3), padding='same', pre=True, relu=True),
+        mode=2, kernels=['maxpool_nhwc_kernel<float4>', 'conv_gemm_wg_kernel<0,64,0>'])
+    c['pool_f32_first_generic_c6'] = lambda: dict(net=ProbeNet(21).conv(6, (4, 5), relu=True).pool(),
+                                                  kernels=['conv_gemm_f32_kernel<64,true>', 'maxpool_nhwc_kernel<float>'])
+    # ---- sigmoid: layers whose shapes the tensor-core engines take still run on the fp32 kernels, which evaluate it
+    c['sigmoid_conv_3x3_c64'] = lambda: dict(net=_first(21).conv(64, (3, 3), act='sigmoid'),
+                                             kernels=['conv_first_direct_kernel', 'conv_gemm_f32_kernel<64,false>'])
+    c['sigmoid_dense_128'] = lambda: dict(net=_first(21).pool().dense(128, act='sigmoid'),
+                                          kernels=['conv_gemm_f32_kernel<128,false>'])
     return c
 
 
