@@ -79,19 +79,31 @@ struct PatchArrays {
     uint8_t *finite;
 };
 
-__global__ void patch_index_kernel(const int32_t *__restrict__ seg_start, const int64_t *__restrict__ seg_off,
-                                   int n_seg, int64_t n, int64_t U, int edge_left, int edge_right,
-                                   int32_t *__restrict__ row0)
+// A range of padded patch indices [start, start + its length) of the recording whose rows begin at row `base` and which
+// has U un-replicated windows.
+struct PatchRange {
+    int64_t base, U;
+    int32_t start;
+};
+
+// first log-mel row of patch p of a range (patch_index_kernel and the host's copy of it)
+__host__ __device__ __forceinline__ int64_t patch_row0(const PatchRange &r, int64_t p, int edge_left, int edge_right)
+{
+    int64_t j = p - (edge_left ? PATCH_LFILL : 0);              // un-replicated window index
+    if (j < 0) j = 0;
+    if (edge_right && j > r.U - 1) j = r.U - 1;
+    return r.base + j * PATCH_HOP;
+}
+
+__global__ void patch_index_kernel(const PatchRange *__restrict__ ranges, const int64_t *__restrict__ seg_off,
+                                   int n_seg, int64_t n, int edge_left, int edge_right, int32_t *__restrict__ row0)
 {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     int lo = 0, hi = n_seg;
     while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (seg_off[mid] <= i) lo = mid; else hi = mid; }
-    const int64_t p = seg_start[lo] + (i - seg_off[lo]);        // padded patch index
-    int64_t j = p - (edge_left ? PATCH_LFILL : 0);              // un-replicated window index
-    if (j < 0) j = 0;
-    if (edge_right && j > U - 1) j = U - 1;
-    row0[i] = (int32_t)(j * PATCH_HOP);
+    const PatchRange r = ranges[lo];
+    row0[i] = (int32_t)patch_row0(r, r.start + (i - seg_off[lo]), edge_left, edge_right);     // padded patch index
 }
 
 // one warp per patch: mean / population std over the 68 x w values (np.mean / np.std, segmenter.py:82)
@@ -382,7 +394,7 @@ extern "C" int64_t iss_cnn_workspace_bytes(const iss_cnn *cnn, int64_t n, int n_
     bytes += align_up((size_t)n, 256);                     // finite
     bytes += align_up((size_t)n * 8 * 4, 256);             // logits [n][<=8]
     bytes += 2 * align_up((size_t)B * cnn->max_act * 4, 256);
-    bytes += align_up((size_t)(n_seg + 1) * 4, 256) + align_up((size_t)(n_seg + 1) * 8, 256);   // segment tables
+    bytes += align_up((size_t)(n_seg + 1) * sizeof(PatchRange), 256) + align_up((size_t)(n_seg + 1) * 8, 256);   // range tables
     bytes += first_y_bytes(cnn, B);                                                               // float64 map of the fused first layer
     return bytes;
 }
@@ -512,28 +524,44 @@ int plan_forward(const iss_cnn *cnn, int mode, const float *mspec, int ld, const
 
 }  // namespace
 
-extern "C" int iss_cnn_forward(iss_ctx *ctx, iss_cnn *cnn, const float *d_mspec, int64_t L, int ld,
-                               int edge_left, int edge_right,
-                               const int32_t *h_seg_start, const int32_t *h_seg_stop, int n_seg,
-                               float *d_probs, void *d_work, int64_t work_bytes, void *stream)
+// The forward pass over n_rec recordings packed in one log-mel buffer of `rows` rows: recording r is rows
+// [h_row_off[r], h_row_off[r] + h_len[r]), and range s covers padded patches [h_seg_start[s], h_seg_stop[s]) of recording
+// h_seg_rec[s] (h_seg_rec == nullptr: all ranges are of recording 0).  The edge flags apply to every recording.
+static int cnn_forward(iss_ctx *ctx, iss_cnn *cnn, const float *d_mspec, int64_t rows, int ld, int edge_left, int edge_right,
+                       const int64_t *h_row_off, const int64_t *h_len, int n_rec, const int32_t *h_seg_rec,
+                       const int32_t *h_seg_start, const int32_t *h_seg_stop, int n_seg,
+                       float *d_probs, void *d_work, int64_t work_bytes, void *stream)
 {
     ISS_REQUIRE(ctx && cnn, ISS_ERR_INVALID, "iss_cnn_forward: NULL handle");
     ISS_REQUIRE(ld >= cnn->in_w, ISS_ERR_INVALID, "iss_cnn_forward: ld=%d < nmel=%d", ld, cnn->in_w);
     if (n_seg <= 0) return ISS_OK;
     ISS_REQUIRE(h_seg_start && h_seg_stop, ISS_ERR_INVALID, "iss_cnn_forward: NULL segment arrays");
-    ISS_REQUIRE(L >= PATCH_H, ISS_ERR_INVALID, "iss_cnn_forward: L=%lld < %d frames (pad short inputs first, segmenter.py:60-65)", (long long)L, PATCH_H);
+    ISS_REQUIRE(rows < (1ll << 31), ISS_ERR_INVALID, "iss_cnn_forward: %lld log-mel rows do not fit 32-bit row indices", (long long)rows);
+    for (int r = 0; r < n_rec; ++r) {
+        const int64_t L = h_len[r];
+        ISS_REQUIRE(L >= PATCH_H, ISS_ERR_INVALID, "iss_cnn_forward: L=%lld < %d frames (pad short inputs first, segmenter.py:60-65)", (long long)L, PATCH_H);
+        ISS_REQUIRE(h_row_off[r] >= 0 && h_row_off[r] + L <= rows, ISS_ERR_INVALID,
+                    "iss_cnn_forward: recording %d = rows [%lld,%lld) outside [0,%lld)", r, (long long)h_row_off[r],
+                    (long long)(h_row_off[r] + L), (long long)rows);
+    }
     ISS_CUDA_OK(cudaSetDevice(ctx->device));
     cudaStream_t st = iss_stream(stream);
-    const int64_t U = (L - PATCH_H) / PATCH_HOP + 1;                      // un-replicated windows
-    const int64_t P = (edge_left ? PATCH_LFILL : 0) + U + (edge_right ? (PATCH_LFILL - 1 + (L % 2)) : 0);
     std::vector<int64_t> off(n_seg + 1);
+    std::vector<PatchRange> rng(n_seg + 1);
     int64_t n = 0;
     for (int s = 0; s < n_seg; ++s) {
+        const int rec = h_seg_rec ? h_seg_rec[s] : 0;
+        ISS_REQUIRE(rec >= 0 && rec < n_rec, ISS_ERR_INVALID, "iss_cnn_forward: range %d names recording %d of %d", s, rec, n_rec);
+        const int64_t L = h_len[rec];
+        const int64_t U = (L - PATCH_H) / PATCH_HOP + 1;                      // un-replicated windows
+        const int64_t P = (edge_left ? PATCH_LFILL : 0) + U + (edge_right ? (PATCH_LFILL - 1 + (L % 2)) : 0);
         ISS_REQUIRE(h_seg_start[s] >= 0 && h_seg_stop[s] >= h_seg_start[s] && h_seg_stop[s] <= P, ISS_ERR_INVALID,
                     "iss_cnn_forward: range %d = [%d,%d) outside [0,%lld)", s, h_seg_start[s], h_seg_stop[s], (long long)P);
+        rng[s] = PatchRange{h_row_off[rec], U, h_seg_start[s]};
         off[s] = n; n += h_seg_stop[s] - h_seg_start[s];
     }
     off[n_seg] = n;
+    rng[n_seg] = PatchRange{0, 0, 0};
     if (n == 0) return ISS_OK;
     ISS_REQUIRE(d_mspec && d_probs && d_work, ISS_ERR_INVALID, "iss_cnn_forward: NULL buffer");
     ISS_REQUIRE(work_bytes >= iss_cnn_workspace_bytes(cnn, n, n_seg), ISS_ERR_INVALID,
@@ -552,7 +580,7 @@ extern "C" int iss_cnn_forward(iss_ctx *ctx, iss_cnn *cnn, const float *d_mspec,
     float *act[2];
     act[0] = reinterpret_cast<float *>(p + o);    o += align_up((size_t)B * cnn->max_act * 4, 256);
     act[1] = reinterpret_cast<float *>(p + o);    o += align_up((size_t)B * cnn->max_act * 4, 256);
-    int32_t *d_seg_start = reinterpret_cast<int32_t *>(p + o); o += align_up((size_t)(n_seg + 1) * 4, 256);
+    PatchRange *d_ranges = reinterpret_cast<PatchRange *>(p + o); o += align_up((size_t)(n_seg + 1) * sizeof(PatchRange), 256);
     int64_t *d_seg_off = reinterpret_cast<int64_t *>(p + o);   o += align_up((size_t)(n_seg + 1) * 8, 256);
     float *d_first_yh = nullptr, *d_first_yl = nullptr, *d_first_coef = nullptr;                // fused first layer (FirstFuse)
     if (first_y_bytes(cnn, B)) {
@@ -566,22 +594,25 @@ extern "C" int iss_cnn_forward(iss_ctx *ctx, iss_cnn *cnn, const float *d_mspec,
     auto host_row0 = [&](int64_t i) -> int64_t {
         int lo = 0, hi = n_seg;
         while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (off[mid] <= i) lo = mid; else hi = mid; }
-        int64_t j = h_seg_start[lo] + (i - off[lo]) - (edge_left ? PATCH_LFILL : 0);
-        if (j < 0) j = 0;
-        if (edge_right && j > U - 1) j = U - 1;
-        return j * PATCH_HOP;
+        return patch_row0(rng[lo], h_seg_start[lo] + (i - off[lo]), edge_left, edge_right);
     };
+    // the fused first layer needs patch rows that never decrease: ranges of one recording ascend, and a range of another
+    // recording starts at or after the last row of the range before it
     bool ranges_ascending = true;
-    for (int s = 1; s < n_seg; ++s) ranges_ascending = ranges_ascending && h_seg_start[s] >= h_seg_stop[s - 1];
+    for (int s = 1; s < n_seg; ++s) {
+        const bool same = !h_seg_rec || h_seg_rec[s] == h_seg_rec[s - 1];
+        ranges_ascending = ranges_ascending && (same ? h_seg_start[s] >= h_seg_stop[s - 1]
+                                                     : (off[s] == 0 || off[s] == n || host_row0(off[s]) >= host_row0(off[s] - 1)));
+    }
     const int mode = iss_get_gemm_mode();
     std::vector<LayerPlan> plan;
     bool fuse_first = false;
     const int prc = plan_forward(cnn, mode, d_mspec, ld, pa, d_first_yh && ranges_ascending, plan, &fuse_first);
     if (prc != ISS_OK) return prc;
-    ISS_CUDA_OK(cudaMemcpyAsync(d_seg_start, h_seg_start, sizeof(int32_t) * n_seg, cudaMemcpyHostToDevice, st));
+    ISS_CUDA_OK(cudaMemcpyAsync(d_ranges, rng.data(), sizeof(PatchRange) * n_seg, cudaMemcpyHostToDevice, st));
     ISS_CUDA_OK(cudaMemcpyAsync(d_seg_off, off.data(), sizeof(int64_t) * (n_seg + 1), cudaMemcpyHostToDevice, st));
 
-    patch_index_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_seg_start, d_seg_off, n_seg, n, U, edge_left, edge_right, pa.row0);
+    patch_index_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_ranges, d_seg_off, n_seg, n, edge_left, edge_right, pa.row0);
     patch_stats_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, st>>>(d_mspec, ld, cnn->in_w, n, pa);
     ISS_CUDA_OK(cudaGetLastError());
     iss_count_launch(2);
@@ -624,16 +655,16 @@ extern "C" int iss_cnn_forward(iss_ctx *ctx, iss_cnn *cnn, const float *d_mspec,
                 if (li == 0 && fuse_first) {
                     // the float64 map of the first layer covers the frames this batch's patches span, if few enough
                     const int64_t f_first = host_row0(b0), f_last = host_row0(b0 + nb - 1);
-                    const int64_t rows = f_last - f_first + Lr.out_h;
-                    if (rows <= first_y_rows(B)) {
-                        const int64_t work = rows * Lr.out_w * (d.cout >> 2);
+                    const int64_t map_rows = f_last - f_first + Lr.out_h;
+                    if (map_rows <= first_y_rows(B)) {
+                        const int64_t work = map_rows * Lr.out_w * (d.cout >> 2);
                         first_linear_kernel<<<(unsigned)((work + 255) / 256), 256, (size_t)d.kh * d.kw * d.cout * sizeof(float), st>>>(
-                            d_mspec, ld, f_first, rows, L, Lr.out_w, d.kh, d.kw, d.cout, a.w, d_first_yh, d_first_yl);
+                            d_mspec, ld, f_first, map_rows, rows, Lr.out_w, d.kh, d.kw, d.cout, a.w, d_first_yh, d_first_yl);
                         first_coef_kernel<<<(unsigned)((nb * d.cout + 255) / 256), 256, 0, st>>>(
                             a.mu, a.sigma, cnn->d_first_S, a.bias, a.pre_scale, a.pre_shift, nb, d.cout, d_first_coef);
                         ISS_CUDA_OK(cudaGetLastError());
                         iss_count_launch(2);
-                        ffuse.Yh = d_first_yh; ffuse.Yl = d_first_yl; ffuse.y_f0 = f_first; ffuse.y_rows = rows;
+                        ffuse.Yh = d_first_yh; ffuse.Yl = d_first_yl; ffuse.y_f0 = f_first; ffuse.y_rows = map_rows;
                         ffuse.row0 = a.row0; ffuse.coef = d_first_coef;
                         ffuse.post_scale = a.post_scale; ffuse.post_shift = a.post_shift; ffuse.flags = a.flags; ffuse.n_img = nb;
                         first_fused = true;                      // nothing stored: layer 1 reads the map
@@ -660,6 +691,26 @@ extern "C" int iss_cnn_forward(iss_ctx *ctx, iss_cnn *cnn, const float *d_mspec,
     ISS_CUDA_OK(cudaGetLastError());
     iss_count_launch();
     return ISS_OK;
+}
+
+extern "C" int iss_cnn_forward(iss_ctx *ctx, iss_cnn *cnn, const float *d_mspec, int64_t L, int ld,
+                               int edge_left, int edge_right,
+                               const int32_t *h_seg_start, const int32_t *h_seg_stop, int n_seg,
+                               float *d_probs, void *d_work, int64_t work_bytes, void *stream)
+{
+    const int64_t zero = 0;
+    return cnn_forward(ctx, cnn, d_mspec, L, ld, edge_left, edge_right, &zero, &L, 1, nullptr, h_seg_start, h_seg_stop, n_seg,
+                       d_probs, d_work, work_bytes, stream);
+}
+
+extern "C" int iss_cnn_forward_multi(iss_ctx *ctx, iss_cnn *cnn, const float *d_mspec, int64_t rows, int ld,
+                                     const int64_t *h_row_off, const int64_t *h_len, int n_rec,
+                                     const int32_t *h_seg_rec, const int32_t *h_seg_start, const int32_t *h_seg_stop, int n_seg,
+                                     float *d_probs, void *d_work, int64_t work_bytes, void *stream)
+{
+    ISS_REQUIRE(n_rec >= 1 && h_row_off && h_len && h_seg_rec, ISS_ERR_INVALID, "iss_cnn_forward_multi: bad recording arguments");
+    return cnn_forward(ctx, cnn, d_mspec, rows, ld, 1, 1, h_row_off, h_len, n_rec, h_seg_rec, h_seg_start, h_seg_stop, n_seg,
+                       d_probs, d_work, work_bytes, stream);
 }
 
 extern "C" int iss_cnn_profile(iss_cnn *cnn, int layer)

@@ -24,6 +24,7 @@
 #include <math.h>
 #include <string.h>
 #include <type_traits>
+#include <vector>
 
 #include "iss_common.cuh"
 
@@ -74,17 +75,36 @@ static_assert(ZPAD * sizeof(float) + 32 * sizeof(double) <= FFT_BUF * 2 * sizeof
 
 __device__ __forceinline__ int bitrev2(int r) { return ((r & 1) << 1) | ((r >> 1) & 1); }
 
+// One recording of a features call.  Its tiles are [tile_off, next recording's tile_off); tile t starts at its frame
+// FR * (t - tile_off), so a recording is tiled exactly as it would be on its own.
+struct FeatRec {
+    const void *pcm;
+    int64_t n_frames;
+    int64_t row_off;                // first mspec row
+    int64_t loge_off;               // first loge entry
+    int64_t tile_off;               // first tile (global block index); entry n_rec holds the total
+    int vec_ok;                     // pcm is 16-byte aligned
+};
+
 template <typename T, int PCM>
 __global__ void __launch_bounds__(NTHREAD, 3)
-sidekit_features_kernel(const void *__restrict__ pcm, int64_t n_samples, int64_t n_frames,
-                        const SidekitTables *__restrict__ tabs, float *__restrict__ mspec,
-                        float *__restrict__ loge, double *__restrict__ partials, int vec_ok)
+sidekit_features_kernel(const FeatRec *__restrict__ recs, int n_rec,
+                        const SidekitTables *__restrict__ tabs, float *__restrict__ mspec_all,
+                        float *__restrict__ loge_all, double *__restrict__ partials)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     Smem<T, PCM> &S = *reinterpret_cast<Smem<T, PCM> *>(smem_raw);
     const int tid = threadIdx.x, lane = tid & 31;
     const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);      // (a value the compiler knows to be warp-uniform: no re-convergence code around the frame loop's shuffles)
-    const int64_t f0 = (int64_t)blockIdx.x * FR;
+    int lo = 0, hi = n_rec;                                      // recs[lo].tile_off <= blockIdx.x < recs[hi].tile_off
+    while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (recs[mid].tile_off <= (int64_t)blockIdx.x) lo = mid; else hi = mid; }
+    const FeatRec &rec = recs[lo];
+    const void *pcm = rec.pcm;
+    const int64_t n_frames = rec.n_frames;
+    const int vec_ok = rec.vec_ok;
+    float *mspec = mspec_all + rec.row_off * ISS_NMEL;
+    float *loge = loge_all + rec.loge_off;
+    const int64_t f0 = ((int64_t)blockIdx.x - rec.tile_off) * FR;
     const int64_t s0 = f0 * ISS_HOP;
     const int nfr = (int)min((int64_t)FR, n_frames - f0);
     const int nsamp = (nfr - 1) * ISS_HOP + ISS_WIN;          // <= TILE_SAMPLES, all < n_samples
@@ -254,10 +274,18 @@ sidekit_features_kernel(const void *__restrict__ pcm, int64_t n_samples, int64_t
     }
 }
 
+// Block b reduces the tiles of recording b (recs == nullptr: the single sequence of ntiles tiles) into stats[b][2];
+// the order depends only on the tile's index within its recording, so a recording gives the same bits in any call.
 __global__ void __launch_bounds__(1024, 1)
-loge_stats_finalize_kernel(const double *__restrict__ partials, int64_t ntiles, double *__restrict__ stats)
+loge_stats_finalize_kernel(const double *__restrict__ partials, const FeatRec *__restrict__ recs, int64_t ntiles,
+                           double *__restrict__ stats)
 {
     __shared__ double ss[1024], sc[1024];
+    if (recs) {
+        partials += 2 * recs[blockIdx.x].tile_off;
+        ntiles = recs[blockIdx.x + 1].tile_off - recs[blockIdx.x].tile_off;
+        stats += 2 * blockIdx.x;
+    }
     double s = 0.0, c = 0.0;
     for (int64_t i = threadIdx.x; i < ntiles; i += 1024) { s += partials[2 * i]; c += partials[2 * i + 1]; }
     ss[threadIdx.x] = s; sc[threadIdx.x] = c;
@@ -317,7 +345,7 @@ extern "C" int iss_loge_stats(iss_ctx *ctx, const float *d_loge, int64_t L, doub
     int rc = ensure_partials(ctx, ntiles);
     if (rc != ISS_OK) return rc;
     loge_tile_partials_kernel<<<(unsigned)((ntiles + 127) / 128), 128, 0, st>>>(d_loge, L, ntiles, ctx->d_partials);
-    loge_stats_finalize_kernel<<<1, 1024, 0, st>>>(ctx->d_partials, ntiles, d_loge_stats);
+    loge_stats_finalize_kernel<<<1, 1024, 0, st>>>(ctx->d_partials, nullptr, ntiles, d_loge_stats);
     ISS_CUDA_OK(cudaGetLastError());
     iss_count_launch(2);
     return ISS_OK;
@@ -396,16 +424,77 @@ extern "C" int iss_sidekit_upload_tables(iss_ctx *ctx, const float *h_fbank, con
 }
 
 template <typename T, int PCM>
-static int launch_features(iss_ctx *ctx, const void *d_pcm, int64_t n_samples, int64_t L, int64_t ntiles,
-                           float *d_mspec, float *d_loge, int vec_ok, cudaStream_t st)
+static int launch_features(iss_ctx *ctx, const FeatRec *d_recs, int n_rec, int64_t ntiles, float *d_mspec, float *d_loge,
+                           cudaStream_t st)
 {
     auto kern = sidekit_features_kernel<T, PCM>;
     const size_t smem = sizeof(Smem<T, PCM>);
     ISS_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kern<<<(unsigned)ntiles, NTHREAD, smem, st>>>(d_pcm, n_samples, L, ctx->d_tables, d_mspec, d_loge,
-                                                   ctx->d_partials, vec_ok);
+    kern<<<(unsigned)ntiles, NTHREAD, smem, st>>>(d_recs, n_rec, ctx->d_tables, d_mspec, d_loge, ctx->d_partials);
     ISS_CUDA_OK(cudaGetLastError());
     iss_count_launch();
+    return ISS_OK;
+}
+
+extern "C" int iss_sidekit_features_multi(iss_ctx *ctx, int n_rec, const void *const *h_pcm, const int64_t *h_n_samples,
+                                          int pcm_format, int fft_precision, float *d_mspec, const int64_t *h_row_off,
+                                          float *d_loge, const int64_t *h_loge_off, double *d_loge_stats, void *stream)
+{
+    ISS_REQUIRE(ctx, ISS_ERR_INVALID, "iss_sidekit_features: ctx is NULL");
+    ISS_REQUIRE(ctx->tables_ready, ISS_ERR_STATE, "iss_sidekit_features: call iss_sidekit_upload_tables first");
+    ISS_REQUIRE(pcm_format == ISS_PCM_F32 || pcm_format == ISS_PCM_S16, ISS_ERR_INVALID, "bad pcm_format %d", pcm_format);
+    ISS_REQUIRE(fft_precision == ISS_FFT_FP32 || fft_precision == ISS_FFT_FP64, ISS_ERR_INVALID, "bad fft_precision %d", fft_precision);
+    ISS_REQUIRE(n_rec >= 1 && h_pcm && h_n_samples && h_row_off && h_loge_off, ISS_ERR_INVALID, "iss_sidekit_features_multi: bad argument");
+    ISS_CUDA_OK(cudaSetDevice(ctx->device));
+    cudaStream_t st = iss_stream(stream);
+    std::vector<FeatRec> recs(n_rec + 1);
+    int64_t ntiles = 0;
+    for (int i = 0; i < n_rec; ++i) {
+        FeatRec &r = recs[i];
+        r.pcm = h_pcm[i];
+        r.n_frames = iss_sidekit_num_frames(h_n_samples[i]);
+        r.row_off = h_row_off[i]; r.loge_off = h_loge_off[i]; r.tile_off = ntiles;
+        r.vec_ok = ((reinterpret_cast<uintptr_t>(r.pcm) & 15) == 0) ? 1 : 0;
+        ISS_REQUIRE(r.n_frames == 0 || r.pcm, ISS_ERR_INVALID, "iss_sidekit_features: NULL buffer (recording %d)", i);
+        ISS_REQUIRE(r.row_off >= 0 && r.loge_off >= 0, ISS_ERR_INVALID, "iss_sidekit_features_multi: negative offset (recording %d)", i);
+        ntiles += (r.n_frames + FR - 1) / FR;
+    }
+    recs[n_rec] = FeatRec{nullptr, 0, 0, 0, ntiles, 0};
+    if (ntiles == 0) {
+        if (d_loge_stats) ISS_CUDA_OK(cudaMemsetAsync(d_loge_stats, 0, 2 * sizeof(double) * n_rec, st));
+        return ISS_OK;
+    }
+    ISS_REQUIRE(d_mspec && d_loge, ISS_ERR_INVALID, "iss_sidekit_features: NULL buffer");
+    ISS_REQUIRE(ntiles < (1ll << 31), ISS_ERR_INVALID, "iss_sidekit_features: signal too long for one call");
+    {
+        const int prc = ensure_partials(ctx, ntiles);
+        if (prc != ISS_OK) return prc;
+    }
+    if (n_rec + 1 > ctx->recs_cap) {
+        if (ctx->d_recs) ISS_CUDA_OK(cudaFree(ctx->d_recs));
+        ctx->d_recs = nullptr; ctx->recs_cap = 0;
+        const int64_t cap = n_rec + 1 + n_rec / 2 + 64;
+        cudaError_t e = cudaMalloc(&ctx->d_recs, (size_t)cap * sizeof(FeatRec));
+        if (e != cudaSuccess) { iss_set_error("cudaMalloc recording table: %s", cudaGetErrorString(e)); return ISS_ERR_NOMEM; }
+        ctx->recs_cap = cap;
+    }
+    const FeatRec *d_recs = reinterpret_cast<const FeatRec *>(ctx->d_recs);
+    ISS_CUDA_OK(cudaMemcpyAsync(ctx->d_recs, recs.data(), sizeof(FeatRec) * (n_rec + 1), cudaMemcpyHostToDevice, st));
+    int rc;
+    if (fft_precision == ISS_FFT_FP32)
+        rc = (pcm_format == ISS_PCM_S16)
+                 ? launch_features<float, ISS_PCM_S16>(ctx, d_recs, n_rec, ntiles, d_mspec, d_loge, st)
+                 : launch_features<float, ISS_PCM_F32>(ctx, d_recs, n_rec, ntiles, d_mspec, d_loge, st);
+    else
+        rc = (pcm_format == ISS_PCM_S16)
+                 ? launch_features<double, ISS_PCM_S16>(ctx, d_recs, n_rec, ntiles, d_mspec, d_loge, st)
+                 : launch_features<double, ISS_PCM_F32>(ctx, d_recs, n_rec, ntiles, d_mspec, d_loge, st);
+    if (rc != ISS_OK) return rc;
+    if (d_loge_stats) {
+        loge_stats_finalize_kernel<<<(unsigned)n_rec, 1024, 0, st>>>(ctx->d_partials, d_recs, 0, d_loge_stats);
+        ISS_CUDA_OK(cudaGetLastError());
+        iss_count_launch();
+    }
     return ISS_OK;
 }
 
@@ -413,39 +502,7 @@ extern "C" int iss_sidekit_features(iss_ctx *ctx, const void *d_pcm, int pcm_for
                                     int fft_precision, float *d_mspec, float *d_loge,
                                     double *d_loge_stats, void *stream)
 {
-    ISS_REQUIRE(ctx, ISS_ERR_INVALID, "iss_sidekit_features: ctx is NULL");
-    ISS_REQUIRE(ctx->tables_ready, ISS_ERR_STATE, "iss_sidekit_features: call iss_sidekit_upload_tables first");
-    ISS_REQUIRE(pcm_format == ISS_PCM_F32 || pcm_format == ISS_PCM_S16, ISS_ERR_INVALID, "bad pcm_format %d", pcm_format);
-    ISS_REQUIRE(fft_precision == ISS_FFT_FP32 || fft_precision == ISS_FFT_FP64, ISS_ERR_INVALID, "bad fft_precision %d", fft_precision);
-    ISS_CUDA_OK(cudaSetDevice(ctx->device));
-    cudaStream_t st = iss_stream(stream);
-    const int64_t L = iss_sidekit_num_frames(n_samples);
-    if (L == 0) {
-        if (d_loge_stats) ISS_CUDA_OK(cudaMemsetAsync(d_loge_stats, 0, 2 * sizeof(double), st));
-        return ISS_OK;
-    }
-    ISS_REQUIRE(d_pcm && d_mspec && d_loge, ISS_ERR_INVALID, "iss_sidekit_features: NULL buffer");
-    const int64_t ntiles = (L + FR - 1) / FR;
-    ISS_REQUIRE(ntiles < (1ll << 31), ISS_ERR_INVALID, "iss_sidekit_features: signal too long for one call");
-    {
-        const int prc = ensure_partials(ctx, ntiles);
-        if (prc != ISS_OK) return prc;
-    }
-    const int vec_ok = ((reinterpret_cast<uintptr_t>(d_pcm) & 15) == 0) ? 1 : 0;
-    int rc;
-    if (fft_precision == ISS_FFT_FP32)
-        rc = (pcm_format == ISS_PCM_S16)
-                 ? launch_features<float, ISS_PCM_S16>(ctx, d_pcm, n_samples, L, ntiles, d_mspec, d_loge, vec_ok, st)
-                 : launch_features<float, ISS_PCM_F32>(ctx, d_pcm, n_samples, L, ntiles, d_mspec, d_loge, vec_ok, st);
-    else
-        rc = (pcm_format == ISS_PCM_S16)
-                 ? launch_features<double, ISS_PCM_S16>(ctx, d_pcm, n_samples, L, ntiles, d_mspec, d_loge, vec_ok, st)
-                 : launch_features<double, ISS_PCM_F32>(ctx, d_pcm, n_samples, L, ntiles, d_mspec, d_loge, vec_ok, st);
-    if (rc != ISS_OK) return rc;
-    if (d_loge_stats) {
-        loge_stats_finalize_kernel<<<1, 1024, 0, st>>>(ctx->d_partials, ntiles, d_loge_stats);
-        ISS_CUDA_OK(cudaGetLastError());
-        iss_count_launch();
-    }
-    return ISS_OK;
+    const int64_t zero = 0;
+    return iss_sidekit_features_multi(ctx, 1, &d_pcm, &n_samples, pcm_format, fft_precision, d_mspec, &zero, d_loge, &zero,
+                                      d_loge_stats, stream);
 }

@@ -62,6 +62,8 @@ extern "C" int iss_ctx_create(int device, iss_ctx **out)
     c->tables_ready = false;
     c->d_partials = nullptr;
     c->partials_cap = 0;
+    c->d_recs = nullptr;
+    c->recs_cap = 0;
     *out = c;
     return ISS_OK;
 }
@@ -72,6 +74,7 @@ extern "C" int iss_ctx_destroy(iss_ctx *ctx)
     cudaSetDevice(ctx->device);
     if (ctx->d_tables) cudaFree(ctx->d_tables);
     if (ctx->d_partials) cudaFree(ctx->d_partials);
+    if (ctx->d_recs) cudaFree(ctx->d_recs);
     delete ctx;
     return ISS_OK;
 }

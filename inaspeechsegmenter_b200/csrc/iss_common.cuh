@@ -60,6 +60,8 @@ struct iss_ctx {
     bool tables_ready;
     double *d_partials;          // per-tile {sum, count} partials of loge
     int64_t partials_cap;        // in tiles
+    void *d_recs;                // per-recording table of a features call (feat_sidekit.cu)
+    int64_t recs_cap;            // in entries
 };
 
 static inline cudaStream_t iss_stream(void *s) { return reinterpret_cast<cudaStream_t>(s); }

@@ -47,6 +47,8 @@ struct VitLayout {
     int alias;                     // 1: every block walks the SAME range seg_off[0..1] (basis chains of a transfer matrix)
                                    // 2: block b walks segment b / 2 with vin / vout slot b (two basis chains per segment)
     int store_bp;                  // 0: scores only
+    int stats_stride;              // energy mode: sequence s thresholds on stats[s * stats_stride ..] (0: one shared pair)
+    const int64_t *out_off;        // [n_seg] first output of each sequence when out_stride > 1, or nullptr (single sequence)
 };
 
 __device__ __forceinline__ bool better(double c, double best)
@@ -68,8 +70,9 @@ viterbi_forward_kernel(const float *__restrict__ src, const double *__restrict__
     double thr = 0.0;
     if (ENERGY) {
         // np.mean(f32 array) is f32; + np.log(ratio) (f64) promotes to f64 (segmenter.py:70)
-        const double cnt = stats[1];
-        const float mean32 = (float)(stats[0] / cnt);          // 0/0 -> NaN like the mean of an empty slice
+        const double *sg = stats + (int64_t)seg * lay.stats_stride;
+        const double cnt = sg[1];
+        const float mean32 = (float)(sg[0] / cnt);          // 0/0 -> NaN like the mean of an empty slice
         thr = (double)mean32 + prm.log_ratio;
     }
     double V[K];
@@ -221,9 +224,10 @@ __global__ void viterbi_chunk_emit_kernel(VitLayout lay, int n_seg, int64_t nchu
     const int64_t a = lc * CH, b = min(a + CH, T);
     const uint8_t *bp = lay.bp + t0;
     unsigned x = lay.cend[c];
+    const int64_t o0 = lay.out_off ? lay.out_off[seg] : t0;         // a single sequence has t0 == 0
     for (int64_t t = b - 1; t >= a; --t) {
-        if (out_stride == 1) states[t0 + t] = (uint8_t)x;
-        else if (t % out_stride == 0) states[(t0 + t) / out_stride] = (uint8_t)x;   // single sequence (t0 == 0)
+        if (out_stride == 1) states[o0 + t] = (uint8_t)x;
+        else if (t % out_stride == 0) states[o0 + t / out_stride] = (uint8_t)x;
         x = (bp[t] >> (2 * x)) & 3;
     }
 }
@@ -484,7 +488,30 @@ extern "C" int64_t iss_viterbi_work_bytes(int64_t total_steps, int n_seg)
     if (total_steps < 0 || n_seg < 0) return -1;
     const int64_t nc = total_steps / CH + n_seg + 1;
     const int64_t chunked = (total_steps / ECH + 2) * 256 + 8192;         // tables of the chunk-parallel energy pass
-    return total_steps + 2 * nc + 2 * (int64_t)sizeof(int64_t) * (n_seg + 1) + n_seg + 8 * 256 + 1024 /* vin/vout/map scratch */ + chunked;
+    return total_steps + 2 * nc + 3 * (int64_t)sizeof(int64_t) * (n_seg + 1) + n_seg + 9 * 256 + 1024 /* vin/vout/map scratch */ + chunked;
+}
+
+// One serial chain per recording: recording r is loge[h_off[r] .. h_off[r+1]) with statistics stats[2r ..] (stats_stride
+// 2) or the one shared pair (stats_stride 0); every out_stride-th state goes to d_states[h_out_off[r] ..], or to
+// d_states[0 ..] for a single recording (h_out_off == nullptr).
+static int energy_chains(iss_ctx *ctx, const float *d_loge, const int64_t *h_off, int n_rec, const double *d_loge_stats,
+                         int stats_stride, const VitParams &prm, int out_stride, const int64_t *h_out_off, uint8_t *d_states,
+                         void *d_work, cudaStream_t st)
+{
+    HostPlan hp; VitLayout lay = {};
+    int rc = make_layout(h_off, n_rec, d_work, hp, lay, st);
+    if (rc != ISS_OK) return rc;
+    lay.store_bp = 1;
+    lay.stats_stride = stats_stride;
+    if (h_out_off) {
+        int64_t *d_out_off = reinterpret_cast<int64_t *>(lay.last + align_up((size_t)n_rec, 256));
+        ISS_CUDA_OK(cudaMemcpyAsync(d_out_off, h_out_off, sizeof(int64_t) * n_rec, cudaMemcpyHostToDevice, st));
+        lay.out_off = d_out_off;
+    }
+    viterbi_forward_kernel<2, true><<<n_rec, 32, 0, st>>>(d_loge, d_loge_stats, prm, lay);
+    ISS_CUDA_OK(cudaGetLastError());
+    iss_count_launch();
+    return run_backtrack(lay, hp, n_rec, out_stride, d_states, st);
 }
 
 extern "C" int iss_energy_viterbi(iss_ctx *ctx, const float *d_loge, int64_t L, const double *d_loge_stats,
@@ -498,19 +525,33 @@ extern "C" int iss_energy_viterbi(iss_ctx *ctx, const float *d_loge, int64_t L, 
     ISS_REQUIRE(d_loge && d_loge_stats && d_states && d_work, ISS_ERR_INVALID, "iss_energy_viterbi: NULL buffer");
     ISS_CUDA_OK(cudaSetDevice(ctx->device));
     cudaStream_t st = iss_stream(stream);
-    const int64_t off[2] = {0, L};
-    HostPlan hp; VitLayout lay = {};
-    int rc = make_layout(off, 1, d_work, hp, lay, st);
-    if (rc != ISS_OK) return rc;
-    lay.store_bp = 1;
     VitParams prm = {};
-    for (int i = 0; i < 2; ++i) for (int j = 0; j < 2; ++j) prm.A[i][j] = h_trans[i * 2 + j];
-    prm.prior = log_prior; prm.emis_hit = h_emis[0]; prm.emis_miss = h_emis[1]; prm.log_ratio = log_ratio;
+    fill_energy_params(prm, h_emis, h_trans, log_prior, log_ratio);
     if (!energy_serial() && L >= 4 * ECH) return energy_viterbi_chunked(ctx, d_loge, L, d_loge_stats, prm, out_stride, d_states, d_work, st);
-    viterbi_forward_kernel<2, true><<<1, 32, 0, st>>>(d_loge, d_loge_stats, prm, lay);
-    ISS_CUDA_OK(cudaGetLastError());
-    iss_count_launch();
-    return run_backtrack(lay, hp, 1, out_stride, d_states, st);
+    const int64_t off[2] = {0, L};
+    return energy_chains(ctx, d_loge, off, 1, d_loge_stats, 0, prm, out_stride, nullptr, d_states, d_work, st);
+}
+
+extern "C" int iss_energy_viterbi_multi(iss_ctx *ctx, const float *d_loge, const int64_t *h_loge_off, int n_rec,
+                                        const double *d_loge_stats, double log_ratio, const double *h_emis,
+                                        const double *h_trans, double log_prior, int out_stride,
+                                        const int64_t *h_out_off, uint8_t *d_states, void *d_work, void *stream)
+{
+    ISS_REQUIRE(ctx && h_emis && h_trans && h_loge_off && h_out_off && n_rec >= 1, ISS_ERR_INVALID, "iss_energy_viterbi_multi: bad argument");
+    ISS_REQUIRE(out_stride >= 1, ISS_ERR_INVALID, "iss_energy_viterbi_multi: out_stride must be >= 1");
+    for (int r = 0; r < n_rec; ++r) {
+        const int64_t L = h_loge_off[r + 1] - h_loge_off[r];
+        ISS_REQUIRE(L >= 0 && L < 4 * ECH, ISS_ERR_INVALID,
+                    "iss_energy_viterbi_multi: recording %d has %lld frames (>= %lld are decoded by iss_energy_viterbi)",
+                    r, (long long)L, (long long)(4 * ECH));
+    }
+    if (h_loge_off[n_rec] == h_loge_off[0]) return ISS_OK;
+    ISS_REQUIRE(d_loge && d_loge_stats && d_states && d_work, ISS_ERR_INVALID, "iss_energy_viterbi_multi: NULL buffer");
+    ISS_CUDA_OK(cudaSetDevice(ctx->device));
+    cudaStream_t st = iss_stream(stream);
+    VitParams prm = {};
+    fill_energy_params(prm, h_emis, h_trans, log_prior, log_ratio);
+    return energy_chains(ctx, d_loge, h_loge_off, n_rec, d_loge_stats, 2, prm, out_stride, h_out_off, d_states, d_work, st);
 }
 
 extern "C" int iss_viterbi_segments(iss_ctx *ctx, const float *d_probs, int K, const int64_t *h_seg_off,

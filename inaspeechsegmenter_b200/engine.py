@@ -91,6 +91,30 @@ class CnnModel:
                                        _stream_ptr(mspec.device, stream)), 'iss_cnn_forward')
         return probs
 
+    def forward_multi(self, mspec, row_off, lens, rec, ranges, stream=None):
+        """Recordings packed in mspec (CUDA float32 [rows, ld]): recording r is rows row_off[r] .. + lens[r]
+        (lens[r] >= 68); range s = ranges[s] = (start, stop) padded patches of recording rec[s], both edges
+        replicated.  Returns CUDA float32 [n, K] as forward() does."""
+        assert mspec.is_cuda and mspec.dtype == torch.float32 and mspec.is_contiguous()
+        rows, ld = mspec.shape
+        row_off = np.ascontiguousarray(row_off, dtype=np.int64)
+        lens = np.ascontiguousarray(lens, dtype=np.int64)
+        rec = np.ascontiguousarray(rec, dtype=np.int32)
+        starts = np.ascontiguousarray([a for a, _ in ranges], dtype=np.int32)
+        stops = np.ascontiguousarray([b for _, b in ranges], dtype=np.int32)
+        n = int((stops - starts).sum()) if len(ranges) else 0
+        probs = torch.empty((n, self.n_classes), dtype=torch.float32, device=mspec.device)
+        if n == 0:
+            return probs
+        lib = _lib.load()
+        work = self.ctx.workspace('cnn', lib.iss_cnn_workspace_bytes(self.handle, n, len(ranges)))
+        _lib.check(lib.iss_cnn_forward_multi(self.ctx.handle, self.handle, _lib.ptr(mspec), rows, ld,
+                                             _lib.ptr(row_off), _lib.ptr(lens), len(lens), _lib.ptr(rec),
+                                             _lib.ptr(starts), _lib.ptr(stops), len(ranges),
+                                             _lib.ptr(probs), _lib.ptr(work), work.numel(),
+                                             _stream_ptr(mspec.device, stream)), 'iss_cnn_forward_multi')
+        return probs
+
     def close(self):
         if self.handle:
             _lib.load().iss_cnn_destroy(self.handle)
@@ -190,6 +214,23 @@ def energy_viterbi(ctx, loge, stats, energy_ratio, out_stride=2, stream=None):
                                       _lib.ptr(_EMIS), _lib.ptr(trans), prior, int(out_stride),
                                       _lib.ptr(states), _lib.ptr(work), _stream_ptr(loge.device, stream)),
                'iss_energy_viterbi')
+    return states
+
+
+def energy_viterbi_multi(ctx, loge, loge_off, stats, energy_ratio, out_off, out_stride=2, stream=None):
+    """energy_viterbi on each recording of a packed loge: recording r is loge[loge_off[r]:loge_off[r+1]] with
+    statistics stats[r] (CUDA float64 [n, 2]); its track goes to states[out_off[r]:out_off[r+1]] -> CUDA uint8."""
+    loge_off = np.ascontiguousarray(loge_off, dtype=np.int64)
+    out_off = np.ascontiguousarray(out_off, dtype=np.int64)
+    n_rec = len(loge_off) - 1
+    states = torch.empty((int(out_off[-1]),), dtype=torch.uint8, device=loge.device)
+    lib = _lib.load()
+    work = ctx.workspace('vit_energy', lib.iss_viterbi_work_bytes(int(loge_off[-1]), n_rec))
+    trans, prior, lr = _energy_consts(energy_ratio)
+    _lib.check(lib.iss_energy_viterbi_multi(ctx.handle, _lib.ptr(loge), _lib.ptr(loge_off), n_rec, _lib.ptr(stats), lr,
+                                            _lib.ptr(_EMIS), _lib.ptr(trans), prior, int(out_stride), _lib.ptr(out_off),
+                                            _lib.ptr(states), _lib.ptr(work), _stream_ptr(loge.device, stream)),
+               'iss_energy_viterbi_multi')
     return states
 
 

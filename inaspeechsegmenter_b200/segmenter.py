@@ -21,7 +21,7 @@ import warnings
 import numpy as np
 import torch
 
-from . import _lib, engine, models
+from . import _lib, engine, models, pack
 from .export_funcs import seg2csv, seg2textgrid
 from .io import media2sig16kmono
 from .sidekit_mfcc import SidekitFrontEnd
@@ -57,6 +57,21 @@ def _to_device_pcm(sig, device):
     except RuntimeError:
         pass
     return host.to(device, non_blocking=True)
+
+
+def _pass_input(sig):
+    """A signal of segment_signals as a 1-D int16 / float32 numpy array or contiguous CUDA tensor (what
+    feats_from_signal would upload)."""
+    if isinstance(sig, torch.Tensor):
+        if sig.is_cuda:
+            if sig.dtype not in (torch.int16, torch.float32):
+                raise TypeError('pcm must be int16 or float32, got %s' % sig.dtype)
+            return sig.contiguous()
+        sig = sig.numpy()
+    sig = np.ascontiguousarray(sig)
+    if sig.dtype not in (np.int16, np.float32):
+        sig = sig.astype(np.float32)
+    return sig
 
 
 def feats_from_signal(sig, device=0, fft_precision=_lib.FFT_FP64, ctx_name='feat', medianame='<array>'):
@@ -127,18 +142,17 @@ class DnnSegmenter:
         assert self.nn.n_classes == len(self.outlabels), (self.nn.n_classes, self.outlabels)
         self.last_probs = None
 
-    def __call__(self, mspec, lseg, difflen=0, edge_left=True, edge_right=True):
-        if isinstance(mspec, np.ndarray):
-            mspec = torch.from_numpy(np.ascontiguousarray(mspec, dtype=np.float32)).to(self.ctx.device)
+    def _ranges(self, lseg, difflen):
         ranges = [(a, b) for lab, a, b in lseg if lab == self.inlabel]
-        ret = []
-        if not ranges:
-            return list(lseg)
-        if difflen > 0:
+        if ranges and difflen > 0:
             # patches[:-int(difflen / 2)] (segmenter.py:150-152): ranges never reach the trimmed tail
             limit = (17 + 1 + 16) - int(difflen / 2)
             assert max(b for _, b in ranges) <= limit, (ranges, limit)
-        probs = self.nn.forward(mspec, ranges, edge_left, edge_right)
+        return ranges
+
+    def _decode(self, probs, ranges, lsegs):
+        """Viterbi over the posteriors of `ranges` (the inlabel segments of the lseg lists, in order), then the
+        relabelled lseg lists."""
         self.last_probs = probs
         seg_off = np.concatenate(([0], np.cumsum([b - a for a, b in ranges]))).astype(np.int64)
         trans = engine.diag_trans_exp(self.viterbi_arg, len(self.outlabels))
@@ -154,15 +168,42 @@ class DnnSegmenter:
                                 % type(self).__name__)
         states = states[:-1]
         k = 0
-        for lab, a, b in lseg:
-            if lab != self.inlabel:
-                ret.append((lab, a, b))
-                continue
-            pred = states[seg_off[k]:seg_off[k + 1]]
-            k += 1
-            for lab2, a2, b2 in _rle(pred):
-                ret.append((self.outlabels[int(lab2)], a2 + a, b2 + a))
-        return ret
+        out = []
+        for lseg in lsegs:
+            ret = []
+            for lab, a, b in lseg:
+                if lab != self.inlabel:
+                    ret.append((lab, a, b))
+                    continue
+                pred = states[seg_off[k]:seg_off[k + 1]]
+                k += 1
+                for lab2, a2, b2 in _rle(pred):
+                    ret.append((self.outlabels[int(lab2)], a2 + a, b2 + a))
+            out.append(ret)
+        return out
+
+    def __call__(self, mspec, lseg, difflen=0, edge_left=True, edge_right=True):
+        if isinstance(mspec, np.ndarray):
+            mspec = torch.from_numpy(np.ascontiguousarray(mspec, dtype=np.float32)).to(self.ctx.device)
+        ranges = self._ranges(lseg, difflen)
+        if not ranges:
+            return list(lseg)
+        probs = self.nn.forward(mspec, ranges, edge_left, edge_right)
+        return self._decode(probs, ranges, [lseg])[0]
+
+    def call_packed(self, mspec, layout, lsegs):
+        """__call__ over the recordings of one pass: mspec holds recording i at rows layout.row_off[i] .. +
+        layout.rows[i] (pack.PassLayout) and lsegs[i] is its segment list.  One CNN call and one Viterbi call for all
+        recordings; ``last_probs`` holds the posteriors of all their inlabel segments, in order."""
+        ranges, rec = [], []
+        for i, lseg in enumerate(lsegs):
+            r = self._ranges(lseg, int(layout.difflen[i]))
+            ranges += r
+            rec += [i] * len(r)
+        if not ranges:
+            return [list(lseg) for lseg in lsegs]
+        probs = self.nn.forward_multi(mspec, layout.row_off, layout.rows, rec, ranges)
+        return self._decode(probs, ranges, lsegs)
 
 
 class SpeechMusic(DnnSegmenter):
@@ -250,6 +291,65 @@ class Segmenter:
         """Extension: segment an in-memory 16 kHz mono signal (numpy int16/float32 or CUDA tensor)."""
         mspec, loge, difflen = feats_from_signal(sig, self.device, self.fft_precision, 'main')
         return self.segment_feats(mspec, loge, difflen, start_sec)
+
+    def segment_signals(self, signals, start_secs=None):
+        """Extension: segment a list of in-memory 16 kHz mono signals (each what ``segment_signal`` accepts) in as few
+        device passes as possible.  Returns one segment list per signal, in input order, equal to
+        ``segment_signal(signals[i], start_secs[i])``.  Host arrays are staged in one pinned buffer per pass; CUDA
+        tensors are read in place.  Signals of 65536 frames (10.9 min) or more go through ``segment_signal``."""
+        n = len(signals)
+        if start_secs is None:
+            start_secs = [0] * n
+        if len(start_secs) != n:
+            raise ValueError('%d signals but %d start times' % (n, len(start_secs)))
+        sigs = [_pass_input(s) for s in signals]
+        pack.check_lengths([s.shape[0] for s in sigs])
+        passes, long_ = pack.plan_passes([s.shape[0] for s in sigs], [str(s.dtype).split('.')[-1] for s in sigs])
+        out = [None] * n
+        for idx in passes:
+            for i, segs in zip(idx, self._segment_pass([sigs[i] for i in idx], [start_secs[i] for i in idx])):
+                out[i] = segs
+        for i in long_:
+            out[i] = self.segment_signal(signals[i], start_secs[i])
+        return out
+
+    def _segment_pass(self, sigs, start_secs):
+        """One device pass over signals of one PCM format, each shorter than pack.LONG_FRAMES frames."""
+        dev = self.ctx.device
+        host = [i for i, s in enumerate(sigs) if isinstance(s, np.ndarray)]
+        itemsize = sigs[0].itemsize if isinstance(sigs[0], np.ndarray) else sigs[0].element_size()
+        layout = pack.PassLayout([s.shape[0] for s in sigs], itemsize)
+        pcms = list(sigs)
+        if host:
+            # one pinned staging buffer, each recording 16-byte aligned, one copy to the device
+            dtype = sigs[host[0]].dtype
+            stage = np.zeros(int(layout.stage_off[-1]), dtype=dtype)
+            for i in host:
+                stage[layout.stage_off[i]:layout.stage_off[i] + sigs[i].shape[0]] = sigs[i]
+            buf = torch.from_numpy(stage)
+            try:
+                buf = buf.pin_memory()
+            except RuntimeError:
+                pass
+            buf = buf.to(dev, non_blocking=True)
+            for i in host:
+                pcms[i] = buf[layout.stage_off[i]:layout.stage_off[i] + sigs[i].shape[0]]
+        mspec, loge, stats = _get_frontend('main', dev.index).multi(pcms, layout, self.fft_precision)
+        for i in np.flatnonzero(layout.difflen > 0):
+            # short media: pad with rows of min(mspec) (segmenter.py:60-65)
+            warnings.warn("media <signal %d> duration is short. Robust results require length of at least 720 "
+                          "milliseconds" % i)
+            a, L = int(layout.row_off[i]), int(layout.frames[i])
+            mspec[a + L:a + pack.PATCH_W] = mspec[a:a + L].min()
+        track = engine.energy_viterbi_multi(self.ctx, loge, layout.loge_off, stats, self.energy_ratio,
+                                            layout.out_off).cpu().numpy()
+        lsegs = [[('noEnergy' if lab == 0 else 'energy', a, b)
+                  for lab, a, b in _rle(track[layout.out_off[i]:layout.out_off[i + 1]])] for i in range(len(sigs))]
+        lsegs = self.vad.call_packed(mspec, layout, lsegs)
+        if self.detect_gender:
+            lsegs = self.gender.call_packed(mspec, layout, lsegs)
+        return [[(lab, start_sec + start * .02, start_sec + stop * .02) for lab, start, stop in lseg]
+                for lseg, start_sec in zip(lsegs, start_secs)]
 
     def batch_process(self, linput, loutput, verbose=False, skipifexist=False, nbtry=1, trydelay=2., output_format='csv'):
         """segmenter.py:297-335 -- same return tuple and message codes."""

@@ -42,6 +42,14 @@ def num_frames(n_samples):
     return int(_lib.load().iss_sidekit_num_frames(int(n_samples)))
 
 
+def _pcm_format(dtype):
+    if dtype == torch.int16:
+        return _lib.PCM_S16
+    if dtype == torch.float32:
+        return _lib.PCM_F32
+    raise TypeError('pcm must be int16 or float32, got %s' % dtype)
+
+
 class SidekitFrontEnd:
     """Owns one library context with the front-end tables uploaded."""
 
@@ -53,16 +61,34 @@ class SidekitFrontEnd:
         _lib.check(lib.iss_sidekit_upload_tables(ctx.handle, _lib.ptr(self._fbank), _lib.ptr(self._window)),
                    'iss_sidekit_upload_tables')
 
+    def multi(self, pcms, layout, fft_precision=_lib.FFT_FP64, stream=None):
+        """pcms: 1-D contiguous CUDA tensors of one dtype (int16 or float32); layout: pack.PassLayout of their sample
+        counts.  Returns (mspec[layout.total_rows, 24] f32 with recording i at rows layout.row_off[i] ..,
+        loge f32 packed at layout.loge_off, stats[n, 2] f64), all on device; each recording's values are those of
+        __call__ on it.  Rows reserved past a recording's frames are left unwritten."""
+        fmt = _pcm_format(pcms[0].dtype)
+        assert all(p.is_cuda and p.dim() == 1 and p.is_contiguous() and p.dtype == pcms[0].dtype for p in pcms)
+        n = len(pcms)
+        dev = pcms[0].device
+        mspec = torch.empty((layout.total_rows, NMEL), dtype=torch.float32, device=dev)
+        loge = torch.empty((int(layout.loge_off[-1]),), dtype=torch.float32, device=dev)
+        stats = torch.empty((n, 2), dtype=torch.float64, device=dev)
+        ptrs = (_lib._c.c_void_p * n)(*[p.data_ptr() for p in pcms])
+        n_samples = np.ascontiguousarray([p.numel() for p in pcms], dtype=np.int64)
+        row_off = np.ascontiguousarray(layout.row_off, dtype=np.int64)
+        loge_off = np.ascontiguousarray(layout.loge_off[:-1], dtype=np.int64)
+        st = stream if stream is not None else torch.cuda.current_stream(dev)
+        _lib.check(_lib.load().iss_sidekit_features_multi(
+            self.ctx.handle, n, ptrs, _lib.ptr(n_samples), fmt, int(fft_precision), _lib.ptr(mspec), _lib.ptr(row_off),
+            _lib.ptr(loge), _lib.ptr(loge_off), _lib.ptr(stats), _lib._c.c_void_p(st.cuda_stream)),
+            'iss_sidekit_features_multi')
+        return mspec, loge, stats
+
     def __call__(self, pcm, fft_precision=_lib.FFT_FP64, stream=None):
         """pcm: CUDA tensor, int16 or float32, 1-D.  Returns (mspec[L,24] f32,
         loge[L] f32, stats[2] f64 = (sum, count) of finite loge), all on device."""
         assert pcm.is_cuda and pcm.dim() == 1 and pcm.is_contiguous()
-        if pcm.dtype == torch.int16:
-            fmt = _lib.PCM_S16
-        elif pcm.dtype == torch.float32:
-            fmt = _lib.PCM_F32
-        else:
-            raise TypeError('pcm must be int16 or float32, got %s' % pcm.dtype)
+        fmt = _pcm_format(pcm.dtype)
         n = pcm.numel()
         L = num_frames(n)
         dev = pcm.device

@@ -39,7 +39,7 @@ typedef struct iss_mlp iss_mlp;
 
 /* ---- library / context ------------------------------------------------- */
 
-#define ISS_ABI_VERSION 2
+#define ISS_ABI_VERSION 3
 int         iss_version(void);               /* == ISS_ABI_VERSION of the header the library was built from */
 const char *iss_last_error(void);
 /* Creates a context bound to CUDA device `device` (one per host thread that
@@ -94,6 +94,16 @@ int iss_sidekit_features(iss_ctx *ctx, const void *d_pcm, int pcm_format, int64_
                          int fft_precision, float *d_mspec, float *d_loge,
                          double *d_loge_stats, void *stream);
 
+/* The same for n_rec recordings in one launch (iss_sidekit_features is its n_rec = 1 case).
+ * Recording r is h_pcm[r] (a DEVICE pointer held in a host array) with h_n_samples[r] samples,
+ * all in one pcm_format; its L_r frames go to the mspec rows h_row_off[r] .. + L_r of d_mspec
+ * ([rows][24]) and to d_loge[h_loge_off[r] .. + L_r], and its {sum, count} to
+ * d_loge_stats[2r], [2r + 1].  Every recording is tiled from its own first frame, so its
+ * mspec, loge and statistics are bit-identical to those of an iss_sidekit_features call on it. */
+int iss_sidekit_features_multi(iss_ctx *ctx, int n_rec, const void *const *h_pcm, const int64_t *h_n_samples,
+                               int pcm_format, int fft_precision, float *d_mspec, const int64_t *h_row_off,
+                               float *d_loge, const int64_t *h_loge_off, double *d_loge_stats, void *stream);
+
 /* Stand-alone version of the {sum, count} reduction over a float32 loge array
  * (e.g. the all-gathered loge of a time-sharded recording): same summation
  * order as the fused reduction inside iss_sidekit_features, hence bit-identical
@@ -124,6 +134,16 @@ int iss_energy_viterbi(iss_ctx *ctx, const float *d_loge, int64_t L, const doubl
                        double log_ratio, const double *h_emis, const double *h_trans,
                        double log_prior, int out_stride, uint8_t *d_states, void *d_work,
                        void *stream);
+/* One independent energy chain per recording, all in one launch: recording r is
+ * d_loge[h_loge_off[r] .. h_loge_off[r+1]) thresholded with d_loge_stats[2r], [2r + 1]
+ * (as iss_sidekit_features_multi writes them); its every out_stride-th state goes to
+ * d_states[h_out_off[r] ..].  d_work: iss_viterbi_work_bytes(h_loge_off[n_rec], n_rec) bytes.
+ * Each chain is decoded serially, so a recording of 4 * 16384 = 65536 frames or more
+ * (which iss_energy_viterbi decodes chunk-parallel) is refused with ISS_ERR_INVALID. */
+int iss_energy_viterbi_multi(iss_ctx *ctx, const float *d_loge, const int64_t *h_loge_off, int n_rec,
+                             const double *d_loge_stats, double log_ratio, const double *h_emis,
+                             const double *h_trans, double log_prior, int out_stride,
+                             const int64_t *h_out_off, uint8_t *d_states, void *d_work, void *stream);
 
 /* Batched decode of CNN posteriors (segmenter.py:167-178): for segment s the
  * rows d_probs[seg_off[s] .. seg_off[s+1]) (float32 [n][K], already carrying
@@ -211,6 +231,17 @@ int iss_cnn_forward(iss_ctx *ctx, iss_cnn *cnn, const float *d_mspec, int64_t L,
                     int edge_left, int edge_right,
                     const int32_t *h_seg_start, const int32_t *h_seg_stop, int n_seg,
                     float *d_probs, void *d_work, int64_t work_bytes, void *stream);
+
+/* The same over n_rec recordings packed in one d_mspec of `rows` rows (iss_cnn_forward is its
+ * one-recording case): recording r is rows h_row_off[r] .. + h_len[r] (h_len[r] >= 68, short
+ * recordings padded first), with edge replication at both of its ends; range s is the padded
+ * patches [h_seg_start[s], h_seg_stop[s]) of recording h_seg_rec[s], so patch p of recording r
+ * is rows h_row_off[r] + 2*clamp(p-17, 0, U_r-1) .. +67.  A patch's posteriors do not depend on
+ * the other patches of the call. */
+int iss_cnn_forward_multi(iss_ctx *ctx, iss_cnn *cnn, const float *d_mspec, int64_t rows, int ld,
+                          const int64_t *h_row_off, const int64_t *h_len, int n_rec,
+                          const int32_t *h_seg_rec, const int32_t *h_seg_start, const int32_t *h_seg_stop, int n_seg,
+                          float *d_probs, void *d_work, int64_t work_bytes, void *stream);
 
 /* ---- K4: VBx / HTK 64-band log-mel front-end + floating CMVN ----------------
  * Replaces get_features(signal) (inaSpeechSegmenter/vbx_segmenter.py:72-89 on top
