@@ -62,7 +62,9 @@ stat_pool_kernel(const float *__restrict__ in, int n_win, int H, int W, int C, f
     const float mean = s1 / (float)W, msq = s2 / (float)W;
     float *o = pooled + (int64_t)w * 2 * C * H;
     o[c * H + h] = mean;
-    o[C * H + c * H + h] = sqrtf(msq - mean * mean + 1e-10f);
+    // msq - mean^2 of a (near-)constant channel rounds to either side of 0: clamped, so that the std is sqrt(1e-10) and not
+    // NaN; the NaN-propagating max (iss_relu) keeps a non-finite activation non-finite
+    o[C * H + c * H + h] = sqrtf(iss_relu(msq - mean * mean) + 1e-10f);
 }
 
 }  // namespace

@@ -232,10 +232,21 @@ class B200BackendExtractor(VBxExtractor):
                                         _stream_ptr(fea.device, stream)), 'iss_resnet_embed')
         return emb
 
+    @staticmethod
+    def _check_range(emb):
+        """On the fp16-split engine, a non-finite embedding means an activation left the fp16 range (|x| < 65504 in the
+        split-half words between its layers): that is an error, not a window to drop.  The fp32-range engines keep
+        the reference's drop-with-warning."""
+        if _lib.load().iss_get_gemm_mode() == _lib.GEMM_TC_F16 and not np.isfinite(emb).all():
+            raise _lib.IssError('B200BackendExtractor: the ResNet returned non-finite x-vectors: an activation left the '
+                                'fp16 range of the default fp16-split GEMM engine; run with ISS_B200_GEMM=tc_ts '
+                                '(3xTF32, fp32 range)')
+        return emb
+
     def get_embedding(self, fea):
         """OnnxBackendExtractor.get_embedding contract (vbx_segmenter.py:262-266): fea [T, 64] -> [256]."""
         t = torch.from_numpy(np.ascontiguousarray(fea, dtype=np.float32)).to(self.ctx.device)
-        return self.embed_windows(t, [0], t.shape[0]).cpu().numpy()[0]
+        return self._check_range(self.embed_windows(t, [0], t.shape[0]).cpu().numpy()[0])
 
     def __call__(self, basename, fea, duration):
         """Same output as VBxExtractor.__call__, windows embedded in GPU batches."""
@@ -245,6 +256,7 @@ class B200BackendExtractor(VBxExtractor):
         plan = window_plan(M)
         reg = [s for s, n, tail in plan if not tail]
         emb = self.embed_windows(fea, reg, WINLEN).cpu().numpy() if reg else np.zeros((0, EMBED_DIM), np.float32)
+        self._check_range(emb)
         out = []
         for i, start in enumerate(reg):
             key = f'{basename}_{start:08}-{(start + WINLEN):08}'
@@ -254,7 +266,7 @@ class B200BackendExtractor(VBxExtractor):
             out.append((key, (round(start / 100.0, 3), round(start / 100.0 + WINLEN / 100.0, 3)), emb[i]))
         for start, n, tail in plan:
             if tail:
-                x = self.embed_windows(fea, [start], n).cpu().numpy()[0]
+                x = self._check_range(self.embed_windows(fea, [start], n).cpu().numpy()[0])
                 key = f'{basename}_{start:08}-{M:08}'
                 if np.isnan(x).any():
                     logger.warning(f'NaN found, not processing: {key}{os.linesep}')
