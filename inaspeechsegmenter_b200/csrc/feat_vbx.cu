@@ -17,8 +17,12 @@
 // Kernel B: sliding 300-frame mean (Kaldi edge handling: the window shifts, it does
 // not shrink), one thread per band, 128-frame chunks: direct sum for the first frame
 // of the chunk, then add/subtract one row per step.
+// Both kernels take a table of recordings (iss_vbx_features_multi): a CTA finds its
+// recording by binary search over the tile / chunk offsets, and every index inside it
+// (padding, dither, tile, CMVN window) is local to that recording.
 #include <math.h>
 #include <string.h>
+#include <vector>
 
 #include "iss_common.cuh"
 
@@ -70,15 +74,41 @@ __device__ __forceinline__ double load_quantised(const void *pcm, int64_t i)
     return trunc((double)reinterpret_cast<const float *>(pcm)[i] * 32768.0);
 }
 
+// One recording of a features call.  Its fbank tiles are [tile_off, next recording's tile_off) and its CMVN chunks
+// [chunk_off, next chunk_off); tile t starts at its frame VFR * (t - tile_off) and chunk c at CMVN_CHUNK * (c - chunk_off),
+// so a recording is tiled, padded, dithered and normalised exactly as it would be on its own.
+struct VbxRec {
+    const void *pcm;
+    int64_t n;                      // samples
+    int64_t M;                      // feature frames
+    int64_t raw_off;                // first row of the float64 scratch
+    int64_t fea_off;                // first output row
+    int64_t tile_off;               // first fbank tile (global block index); entry n_rec holds the total
+    int64_t chunk_off;              // first CMVN chunk (global block index); entry n_rec holds the total
+};
+
+// recs[lo].off <= b < recs[hi].off (recordings without frames own no block)
+template <int64_t VbxRec::*OFF>
+__device__ __forceinline__ const VbxRec &find_rec(const VbxRec *__restrict__ recs, int n_rec, int64_t b)
+{
+    int lo = 0, hi = n_rec;
+    while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (recs[mid].*OFF <= b) lo = mid; else hi = mid; }
+    return recs[lo];
+}
+
 template <int PCM>
 __global__ void __launch_bounds__(VNTHREAD, 2)
-vbx_fbank_kernel(const void *__restrict__ pcm, const double *__restrict__ dither, int64_t n, int64_t M,
-                 const VbxTables *__restrict__ tabs, double *__restrict__ raw)
+vbx_fbank_kernel(const VbxRec *__restrict__ recs, int n_rec, const double *__restrict__ dither,
+                 const VbxTables *__restrict__ tabs, double *__restrict__ raw_all)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     VSmem &S = *reinterpret_cast<VSmem *>(smem_raw);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int64_t f0 = (int64_t)blockIdx.x * VFR;
+    const VbxRec &rec = find_rec<&VbxRec::tile_off>(recs, n_rec, blockIdx.x);
+    const void *pcm = rec.pcm;
+    const int64_t n = rec.n, M = rec.M;
+    double *raw = raw_all + rec.raw_off * VBANDS;
+    const int64_t f0 = ((int64_t)blockIdx.x - rec.tile_off) * VFR;
     const int nfr = (int)min((int64_t)VFR, M - f0);
     const int nsamp = (nfr - 1) * ISS_HOP + ISS_WIN;
     const int64_t p0 = f0 * ISS_HOP;                    // first index in the mirror-padded signal
@@ -154,11 +184,16 @@ vbx_fbank_kernel(const void *__restrict__ pcm, const double *__restrict__ dither
     }
 }
 
-__global__ void __launch_bounds__(VBANDS)
-vbx_cmvn_kernel(const double *__restrict__ raw, int64_t M, float *__restrict__ fea)
+// (32 CTAs of 64 threads per SM, as before the record table: the lookup fits the 32 registers without spills)
+__global__ void __launch_bounds__(VBANDS, 32)
+vbx_cmvn_kernel(const VbxRec *__restrict__ recs, int n_rec, const double *__restrict__ raw_all, float *__restrict__ fea_all)
 {
     const int band = threadIdx.x;
-    const int64_t t0 = (int64_t)blockIdx.x * CMVN_CHUNK;
+    const VbxRec &rec = find_rec<&VbxRec::chunk_off>(recs, n_rec, blockIdx.x);
+    const int64_t M = rec.M;                            // the window never leaves this recording's rows
+    const double *raw = raw_all + rec.raw_off * VBANDS;
+    float *fea = fea_all + rec.fea_off * VBANDS;
+    const int64_t t0 = ((int64_t)blockIdx.x - rec.chunk_off) * CMVN_CHUNK;
     const int64_t t1 = min(t0 + CMVN_CHUNK, M);
     const int64_t wl = min(M, (int64_t)CMVN_WIN);
     auto wstart = [&](int64_t t) { return max(min(t - CMVN_LC, M - wl), (int64_t)0); };
@@ -224,31 +259,63 @@ extern "C" int64_t iss_vbx_work_bytes(int64_t n_samples)
     return iss_vbx_num_frames(n_samples) * VBANDS * (int64_t)sizeof(double) + 256;
 }
 
-extern "C" int iss_vbx_features(iss_ctx *ctx, const void *d_pcm, int pcm_format, int64_t n_samples,
-                                const double *d_dither, float *d_fea, void *d_work, void *stream)
+extern "C" int iss_vbx_features_multi(iss_ctx *ctx, int n_rec, const void *const *h_pcm, const int64_t *h_n_samples,
+                                      int pcm_format, const double *d_dither, float *d_fea, const int64_t *h_fea_off,
+                                      void *d_work, void *stream)
 {
     ISS_REQUIRE(ctx, ISS_ERR_INVALID, "iss_vbx_features: ctx is NULL");
     ISS_REQUIRE(ctx->device < 64 && g_vbx_tables[ctx->device], ISS_ERR_STATE, "iss_vbx_features: call iss_vbx_upload_tables first");
     ISS_REQUIRE(pcm_format == ISS_PCM_F32 || pcm_format == ISS_PCM_S16, ISS_ERR_INVALID, "bad pcm_format %d", pcm_format);
-    const int64_t M = iss_vbx_num_frames(n_samples);
-    if (M == 0) return ISS_OK;
-    ISS_REQUIRE(d_pcm && d_fea && d_work, ISS_ERR_INVALID, "iss_vbx_features: NULL buffer");
+    ISS_REQUIRE(n_rec >= 1 && h_pcm && h_n_samples && h_fea_off, ISS_ERR_INVALID, "iss_vbx_features_multi: bad argument");
+    std::vector<VbxRec> recs(n_rec + 1);
+    int64_t rows = 0, ntiles = 0, nchunks = 0;
+    for (int i = 0; i < n_rec; ++i) {
+        VbxRec &r = recs[i];
+        r.pcm = h_pcm[i];
+        r.n = h_n_samples[i];
+        r.M = iss_vbx_num_frames(r.n);
+        r.raw_off = rows; r.fea_off = h_fea_off[i]; r.tile_off = ntiles; r.chunk_off = nchunks;
+        ISS_REQUIRE(r.M == 0 || r.pcm, ISS_ERR_INVALID, "iss_vbx_features: NULL buffer (recording %d)", i);
+        ISS_REQUIRE(r.fea_off >= 0, ISS_ERR_INVALID, "iss_vbx_features_multi: negative offset (recording %d)", i);
+        rows += r.M;
+        ntiles += (r.M + VFR - 1) / VFR;
+        nchunks += (r.M + CMVN_CHUNK - 1) / CMVN_CHUNK;
+    }
+    recs[n_rec] = VbxRec{nullptr, 0, 0, rows, 0, ntiles, nchunks};
+    if (rows == 0) return ISS_OK;
+    ISS_REQUIRE(d_fea && d_work, ISS_ERR_INVALID, "iss_vbx_features: NULL buffer");
+    ISS_REQUIRE(ntiles < (1ll << 31), ISS_ERR_INVALID, "iss_vbx_features: signal too long for one call");
     ISS_CUDA_OK(cudaSetDevice(ctx->device));
     cudaStream_t st = iss_stream(stream);
+    if (n_rec + 1 > ctx->vbx_recs_cap) {
+        if (ctx->d_vbx_recs) ISS_CUDA_OK(cudaFree(ctx->d_vbx_recs));
+        ctx->d_vbx_recs = nullptr; ctx->vbx_recs_cap = 0;
+        const int64_t cap = n_rec + 1 + n_rec / 2 + 64;
+        cudaError_t e = cudaMalloc(&ctx->d_vbx_recs, (size_t)cap * sizeof(VbxRec));
+        if (e != cudaSuccess) { iss_set_error("cudaMalloc recording table: %s", cudaGetErrorString(e)); return ISS_ERR_NOMEM; }
+        ctx->vbx_recs_cap = cap;
+    }
+    const VbxRec *d_recs = reinterpret_cast<const VbxRec *>(ctx->d_vbx_recs);
+    ISS_CUDA_OK(cudaMemcpyAsync(ctx->d_vbx_recs, recs.data(), sizeof(VbxRec) * (n_rec + 1), cudaMemcpyHostToDevice, st));
     double *raw = reinterpret_cast<double *>(d_work);
-    const int64_t ntiles = (M + VFR - 1) / VFR;
-    ISS_REQUIRE(ntiles < (1ll << 31), ISS_ERR_INVALID, "iss_vbx_features: signal too long for one call");
     const size_t smem = sizeof(VSmem);
     if (pcm_format == ISS_PCM_S16) {
         ISS_CUDA_OK(cudaFuncSetAttribute(vbx_fbank_kernel<ISS_PCM_S16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        vbx_fbank_kernel<ISS_PCM_S16><<<(unsigned)ntiles, VNTHREAD, smem, st>>>(d_pcm, d_dither, n_samples, M, g_vbx_tables[ctx->device], raw);
+        vbx_fbank_kernel<ISS_PCM_S16><<<(unsigned)ntiles, VNTHREAD, smem, st>>>(d_recs, n_rec, d_dither, g_vbx_tables[ctx->device], raw);
     } else {
         ISS_CUDA_OK(cudaFuncSetAttribute(vbx_fbank_kernel<ISS_PCM_F32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        vbx_fbank_kernel<ISS_PCM_F32><<<(unsigned)ntiles, VNTHREAD, smem, st>>>(d_pcm, d_dither, n_samples, M, g_vbx_tables[ctx->device], raw);
+        vbx_fbank_kernel<ISS_PCM_F32><<<(unsigned)ntiles, VNTHREAD, smem, st>>>(d_recs, n_rec, d_dither, g_vbx_tables[ctx->device], raw);
     }
     ISS_CUDA_OK(cudaGetLastError());
-    vbx_cmvn_kernel<<<(unsigned)((M + CMVN_CHUNK - 1) / CMVN_CHUNK), VBANDS, 0, st>>>(raw, M, d_fea);
+    vbx_cmvn_kernel<<<(unsigned)nchunks, VBANDS, 0, st>>>(d_recs, n_rec, raw, d_fea);
     ISS_CUDA_OK(cudaGetLastError());
     iss_count_launch(2);
     return ISS_OK;
+}
+
+extern "C" int iss_vbx_features(iss_ctx *ctx, const void *d_pcm, int pcm_format, int64_t n_samples,
+                                const double *d_dither, float *d_fea, void *d_work, void *stream)
+{
+    const int64_t zero = 0;
+    return iss_vbx_features_multi(ctx, 1, &d_pcm, &n_samples, pcm_format, d_dither, d_fea, &zero, d_work, stream);
 }

@@ -64,6 +64,8 @@ extern "C" int iss_ctx_create(int device, iss_ctx **out)
     c->partials_cap = 0;
     c->d_recs = nullptr;
     c->recs_cap = 0;
+    c->d_vbx_recs = nullptr;
+    c->vbx_recs_cap = 0;
     *out = c;
     return ISS_OK;
 }
@@ -75,6 +77,7 @@ extern "C" int iss_ctx_destroy(iss_ctx *ctx)
     if (ctx->d_tables) cudaFree(ctx->d_tables);
     if (ctx->d_partials) cudaFree(ctx->d_partials);
     if (ctx->d_recs) cudaFree(ctx->d_recs);
+    if (ctx->d_vbx_recs) cudaFree(ctx->d_vbx_recs);
     delete ctx;
     return ISS_OK;
 }

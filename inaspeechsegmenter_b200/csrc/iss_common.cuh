@@ -62,6 +62,8 @@ struct iss_ctx {
     int64_t partials_cap;        // in tiles
     void *d_recs;                // per-recording table of a features call (feat_sidekit.cu)
     int64_t recs_cap;            // in entries
+    void *d_vbx_recs;            // per-recording table of a VBx features call (feat_vbx.cu)
+    int64_t vbx_recs_cap;        // in entries
 };
 
 static inline cudaStream_t iss_stream(void *s) { return reinterpret_cast<cudaStream_t>(s); }

@@ -89,3 +89,56 @@ def patch_row0(L, p):
 def num_patches(L):
     """Padded patches of a recording of L >= 68 frames: 17 + U + 16 + L % 2."""
     return PATCH_LFILL + (L - PATCH_W) // 2 + 1 + PATCH_LFILL - 1 + L % 2
+
+
+# ---- VBx x-vector windows of VoiceFemininityScoring.score_signals ---------------------------------------------------
+VBX_PADL, VBX_PADR = 120, 200      # mirror padding of get_features (feat_vbx.cu VPADL / VPADR)
+VBX_STEP, VBX_WINLEN = 24, 144     # x-vector window hop and length in frames (vbx_segmenter.STEP / WINLEN)
+VBX_MIN_TAIL = 10                  # a shorter remainder gets no tail window
+
+
+def vbx_num_frames(n_samples):
+    """VBx feature frames of a recording of n_samples samples (iss_vbx_num_frames): 0 below 200 samples."""
+    return (n_samples + VBX_PADL + VBX_PADR - WIN) // HOP + 1 if n_samples >= VBX_PADR else 0
+
+
+def window_plan(M):
+    """(start, length, is_tail) for every window of VBxExtractor.__call__ on M feature frames (vbx_segmenter.py:222-243):
+    regular windows every 24 frames while one more fits strictly inside, then a tail from the next hop to the end if it
+    holds at least 10 frames."""
+    plan, start = [], 0
+    for start in range(0, M - VBX_WINLEN, VBX_STEP):
+        plan.append((start, VBX_WINLEN, False))
+    if M - start - VBX_STEP >= VBX_MIN_TAIL:
+        plan.append((start + VBX_STEP, M - (start + VBX_STEP), True))
+    return plan
+
+
+class VbxPlan:
+    """Where the VBx features and x-vector windows of a list of recordings live when their features are packed in one
+    [fea_off[-1], 64] buffer (int64 numpy arrays):
+      frames    M_i;  fea_off  first feature row of recording i (n + 1)
+      reg_start packed first row of every regular 144-frame window, recordings in order and each one's windows in order;
+      reg_rec   its recording;  reg_off  first regular window of recording i (n + 1)
+      tails     {length: (recordings, packed starts)}: the tail windows grouped by length, in recording order;
+      tail_pos  position of recording i's tail in its length group, -1 if it has none
+    """
+
+    def __init__(self, n_samples):
+        self.frames = np.array([vbx_num_frames(int(n)) for n in n_samples], dtype=np.int64)
+        self.fea_off = _starts(self.frames, total=True)
+        self.plans = [window_plan(int(M)) for M in self.frames]
+        reg = [[s for s, _, tail in p if not tail] for p in self.plans]
+        self.reg_off = _starts([len(r) for r in reg], total=True)
+        self.reg_start = np.array([self.fea_off[i] + s for i, r in enumerate(reg) for s in r], dtype=np.int64)
+        self.reg_rec = np.repeat(np.arange(len(reg), dtype=np.int64), [len(r) for r in reg])
+        groups = {}
+        self.tail_pos = np.full(len(self.plans), -1, dtype=np.int64)
+        for i, p in enumerate(self.plans):
+            for s, n, tail in p:
+                if tail:
+                    g = groups.setdefault(n, ([], []))
+                    self.tail_pos[i] = len(g[0])
+                    g[0].append(i)
+                    g[1].append(self.fea_off[i] + s)
+        self.tails = {n: (np.array(r, dtype=np.int64), np.array(s, dtype=np.int64)) for n, (r, s) in sorted(groups.items())}

@@ -74,6 +74,27 @@ def _pass_input(sig):
     return sig
 
 
+def _stage_pass(sigs, stage_off, dev):
+    """Device views of the signals of one pass (numpy arrays or CUDA tensors of one dtype): CUDA tensors are used in
+    place, host arrays are copied into one pinned staging buffer at stage_off (pack.PassLayout: each recording 16-byte
+    aligned) and uploaded in one copy."""
+    host = [i for i, s in enumerate(sigs) if isinstance(s, np.ndarray)]
+    pcms = list(sigs)
+    if host:
+        stage = np.zeros(int(stage_off[-1]), dtype=sigs[host[0]].dtype)
+        for i in host:
+            stage[stage_off[i]:stage_off[i] + sigs[i].shape[0]] = sigs[i]
+        buf = torch.from_numpy(stage)
+        try:
+            buf = buf.pin_memory()
+        except RuntimeError:
+            pass
+        buf = buf.to(dev, non_blocking=True)
+        for i in host:
+            pcms[i] = buf[stage_off[i]:stage_off[i] + sigs[i].shape[0]]
+    return pcms
+
+
 def feats_from_signal(sig, device=0, fft_precision=_lib.FFT_FP64, ctx_name='feat', medianame='<array>'):
     """(mspec, loge, difflen) on the device from a host (or device) 16 kHz mono
     signal: the body of ``_media2feats`` after decoding (segmenter.py:53-67)."""
@@ -316,24 +337,9 @@ class Segmenter:
     def _segment_pass(self, sigs, start_secs):
         """One device pass over signals of one PCM format, each shorter than pack.LONG_FRAMES frames."""
         dev = self.ctx.device
-        host = [i for i, s in enumerate(sigs) if isinstance(s, np.ndarray)]
         itemsize = sigs[0].itemsize if isinstance(sigs[0], np.ndarray) else sigs[0].element_size()
         layout = pack.PassLayout([s.shape[0] for s in sigs], itemsize)
-        pcms = list(sigs)
-        if host:
-            # one pinned staging buffer, each recording 16-byte aligned, one copy to the device
-            dtype = sigs[host[0]].dtype
-            stage = np.zeros(int(layout.stage_off[-1]), dtype=dtype)
-            for i in host:
-                stage[layout.stage_off[i]:layout.stage_off[i] + sigs[i].shape[0]] = sigs[i]
-            buf = torch.from_numpy(stage)
-            try:
-                buf = buf.pin_memory()
-            except RuntimeError:
-                pass
-            buf = buf.to(dev, non_blocking=True)
-            for i in host:
-                pcms[i] = buf[layout.stage_off[i]:layout.stage_off[i] + sigs[i].shape[0]]
+        pcms = _stage_pass(sigs, layout.stage_off, dev)
         mspec, loge, stats = _get_frontend('main', dev.index).multi(pcms, layout, self.fft_precision)
         for i in np.flatnonzero(layout.difflen > 0):
             # short media: pad with rows of min(mspec) (segmenter.py:60-65)

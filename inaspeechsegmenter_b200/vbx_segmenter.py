@@ -17,8 +17,9 @@ from abc import ABC, abstractmethod
 import numpy as np
 import torch
 
-from . import _lib
+from . import _lib, pack
 from .engine import Context, _stream_ptr
+from .pack import window_plan  # noqa: F401  (kept importable from this module)
 
 logger = logging.getLogger(__name__)
 
@@ -94,6 +95,28 @@ class VbxFrontEnd:
         _lib.check(lib.iss_vbx_features(self.ctx.handle, _lib.ptr(pcm), fmt, n, _lib.ptr(d), _lib.ptr(fea),
                                         _lib.ptr(work), _stream_ptr(pcm.device, stream)), 'iss_vbx_features')
         return fea
+
+    def multi(self, pcms, dither=True, stream=None):
+        """pcms: 1-D contiguous CUDA tensors of one dtype (int16 or float32) -> (CUDA float32 [sum M_i, 64], int64 numpy
+        row offsets [n + 1]): recording i's features are rows off[i] .. off[i + 1], equal to __call__ on it."""
+        assert len(pcms) and all(p.is_cuda and p.dim() == 1 and p.is_contiguous() and p.dtype == pcms[0].dtype for p in pcms)
+        fmt = {torch.int16: _lib.PCM_S16, torch.float32: _lib.PCM_F32}[pcms[0].dtype]
+        lib = _lib.load()
+        n = len(pcms)
+        n_samples = np.ascontiguousarray([p.numel() for p in pcms], dtype=np.int64)
+        off = pack._starts([pack.vbx_num_frames(int(k)) for k in n_samples], total=True)
+        dev = pcms[0].device
+        fea = torch.empty((int(off[-1]), FEAT_DIM), dtype=torch.float32, device=dev)
+        if off[-1] == 0:
+            return fea, off
+        work = self.ctx.workspace('vbx', FEAT_DIM * 8 * int(off[-1]) + 256)      # float64 log-fbank rows + 256
+        d = self.dither.get(int(n_samples.max())) if dither else None
+        ptrs = (ctypes.c_void_p * n)(*[p.data_ptr() for p in pcms])
+        fea_off = np.ascontiguousarray(off[:-1])
+        _lib.check(lib.iss_vbx_features_multi(self.ctx.handle, n, ptrs, _lib.ptr(n_samples), fmt, _lib.ptr(d), _lib.ptr(fea),
+                                              _lib.ptr(fea_off), _lib.ptr(work), _stream_ptr(dev, stream)),
+                   'iss_vbx_features_multi')
+        return fea, off
 
 
 _frontends = {}
@@ -171,16 +194,6 @@ class VBxExtractor(ABC):
         return out
 
 
-def window_plan(M):
-    """(start, length, is_tail) for every window of VBxExtractor.__call__ (vbx_segmenter.py:222-243)."""
-    plan, start = [], 0
-    for start in range(0, M - WINLEN, STEP):
-        plan.append((start, WINLEN, False))
-    if M - start - STEP >= 10:
-        plan.append((start + STEP, M - (start + STEP), True))
-    return plan
-
-
 class B200BackendExtractor(VBxExtractor):
     """ResNet101 x-vector extractor on libiss_b200 (K5)."""
 
@@ -233,14 +246,14 @@ class B200BackendExtractor(VBxExtractor):
         return emb
 
     @staticmethod
-    def _check_range(emb):
+    def _check_range(emb, what=''):
         """On the fp16-split engine, a non-finite embedding means an activation left the fp16 range (|x| < 65504 in the
         split-half words between its layers): that is an error, not a window to drop.  The fp32-range engines keep
-        the reference's drop-with-warning."""
+        the reference's drop-with-warning.  `what` names the recording in the message."""
         if _lib.load().iss_get_gemm_mode() == _lib.GEMM_TC_F16 and not np.isfinite(emb).all():
-            raise _lib.IssError('B200BackendExtractor: the ResNet returned non-finite x-vectors: an activation left the '
+            raise _lib.IssError('B200BackendExtractor: the ResNet returned non-finite x-vectors%s: an activation left the '
                                 'fp16 range of the default fp16-split GEMM engine; run with ISS_B200_GEMM=tc_ts '
-                                '(3xTF32, fp32 range)')
+                                '(3xTF32, fp32 range)' % what)
         return emb
 
     def get_embedding(self, fea):
@@ -256,23 +269,56 @@ class B200BackendExtractor(VBxExtractor):
         plan = window_plan(M)
         reg = [s for s, n, tail in plan if not tail]
         emb = self.embed_windows(fea, reg, WINLEN).cpu().numpy() if reg else np.zeros((0, EMBED_DIM), np.float32)
-        self._check_range(emb)
+        tail = lambda start, n: self.embed_windows(fea, [start], n).cpu().numpy()[0]     # noqa: E731
+        return self._xvectors(basename, M, duration, plan, emb, tail)
+
+    def _xvectors(self, basename, M, duration, plan, emb, tail, what=''):
+        """The per-window bookkeeping of __call__ for one recording of M frames: emb holds the x-vectors of the plan's
+        regular windows, in order, and tail(start, n) returns the tail window's."""
+        self._check_range(emb, what)
         out = []
-        for i, start in enumerate(reg):
+        for i, (start, _, _) in enumerate(w for w in plan if not w[2]):
             key = f'{basename}_{start:08}-{(start + WINLEN):08}'
             if np.isnan(emb[i]).any():
                 logger.warning(f'NaN found, not processing: {key}{os.linesep}')
                 continue
             out.append((key, (round(start / 100.0, 3), round(start / 100.0 + WINLEN / 100.0, 3)), emb[i]))
-        for start, n, tail in plan:
-            if tail:
-                x = self._check_range(self.embed_windows(fea, [start], n).cpu().numpy()[0])
+        for start, n, is_tail in plan:
+            if is_tail:
+                x = self._check_range(tail(start, n), what)
                 key = f'{basename}_{start:08}-{M:08}'
                 if np.isnan(x).any():
                     logger.warning(f'NaN found, not processing: {key}{os.linesep}')
                 else:
                     out.append((key, (round(start / 100.0, 3), round(duration, 3)), x))
         return [(key, seg, x * 10) for key, seg, x in out]
+
+    def embed_packed(self, fea, plan, stream=None):
+        """The x-vectors of every window of the recordings packed in fea (CUDA float32 [rows, 64]) by plan
+        (pack.VbxPlan): one embed_windows call for all regular windows, one per distinct tail length, one copy back.
+        Returns (regular [len(plan.reg_start), 256], {tail length: [windows, 256]}), numpy float32."""
+        parts = [self.embed_windows(fea, plan.reg_start, WINLEN, stream)]
+        parts += [self.embed_windows(fea, starts, n, stream) for n, (_, starts) in plan.tails.items()]
+        host = torch.cat(parts).cpu().numpy()
+        reg, k, tails = host[:len(plan.reg_start)], len(plan.reg_start), {}
+        for n, (recs, _) in plan.tails.items():
+            tails[n] = host[k:k + len(recs)]
+            k += len(recs)
+        return reg, tails
+
+    def packed_xvectors(self, plan, emb, i, basename, duration, what=''):
+        """__call__'s result for recording i of a pack.VbxPlan, from the embed_packed output emb."""
+        reg, tails = emb
+        M = int(plan.frames[i])
+        tail = lambda start, n: tails[n][plan.tail_pos[i]]     # noqa: E731
+        return self._xvectors(basename, M, duration, plan.plans[i], reg[plan.reg_off[i]:plan.reg_off[i + 1]], tail, what)
+
+    def call_packed(self, fea, plan, basenames, durations, stream=None):
+        """__call__ on every recording of fea packed by plan (pack.VbxPlan), each with its basename and duration: the same
+        lists, in order.  The engine-3 range error names the first failing recording's index."""
+        emb = self.embed_packed(fea, plan, stream)
+        return [self.packed_xvectors(plan, emb, i, basenames[i], durations[i], ' (signal %d)' % i)
+                for i in range(len(plan.frames))]
 
 
 # ------------------------------------------------------------------ VoiceFemininityScoring (vbx_segmenter.py:28-202)
@@ -376,6 +422,70 @@ class VoiceFemininityScoring:
             gender_pred = np.squeeze(gender_pred)
         g = [(seg[0], seg[1], p) for (_, seg, _), p in zip(x_vectors, gender_pred)]
         return get_femininity_score(g), speech_duration, len(g)
+
+    def score_signals(self, signals, basename='signal'):
+        """score_signal on each of a list of signals (what score_signal takes, or 1-D int16 / float32 CUDA tensors, read in
+        place) in as few device passes as possible: one (score, speech_duration, nb_vectors) per signal, in input order,
+        equal to score_signal(signals[i]).  Per pass of pack.plan_passes, host arrays are staged and uploaded once, the VAD
+        runs as Segmenter.segment_signals, the VBx features of the recordings with speech as one K4 launch pair, their
+        x-vectors as one ResNet call for all regular windows plus one per tail length, and the MLP once.  Signals of
+        pack.LONG_FRAMES frames or more go through score_signal.  If score_signal would raise for some signals, the
+        exception of the first of them is raised."""
+        from .segmenter import _pass_input
+        sigs = [_pass_input(s) for s in signals]
+        pack.check_lengths([s.shape[0] for s in sigs])
+        passes, long_ = pack.plan_passes([s.shape[0] for s in sigs], [str(s.dtype).split('.')[-1] for s in sigs])
+        out = [None] * len(sigs)
+        for idx in passes:
+            for i, r in zip(idx, self._score_pass([sigs[i] for i in idx], idx, basename)):
+                out[i] = r
+        for i in long_:
+            sig = signals[i].cpu().numpy() if isinstance(signals[i], torch.Tensor) else signals[i]
+            try:
+                out[i] = self.score_signal(sig, basename)
+            except Exception as e:          # raised below, in input order
+                out[i] = e
+        for r in out:
+            if isinstance(r, Exception):
+                raise r
+        return out
+
+    def _score_pass(self, sigs, idx, basename):
+        """One pass of score_signals over signals of one PCM format (idx: their input indices).  A recording for which
+        score_signal would raise gets the exception as its result."""
+        from .segmenter import _stage_pass
+        itemsize = sigs[0].itemsize if isinstance(sigs[0], np.ndarray) else sigs[0].element_size()
+        pcms = _stage_pass(sigs, pack.PassLayout([s.shape[0] for s in sigs], itemsize).stage_off, self.ctx.device)
+        speech = [[(b, e) for lab, b, e in segs if lab == 'speech'] for segs in self.vad.segment_signals(pcms)]
+        out = [(None, sum(e - b for b, e in sp), 0) for sp in speech]
+        live = [k for k, sp in enumerate(speech) if out[k][1]]
+        if not live:
+            return out
+        fea, _ = self.frontend.multi([pcms[k] for k in live])
+        plan = pack.VbxPlan([pcms[k].numel() for k in live])
+        emb = self.xvector_model.embed_packed(fea, plan)
+        kept = {}
+        for j, k in enumerate(live):
+            try:
+                xv = self.xvector_model.packed_xvectors(plan, emb, j, basename, pcms[k].numel() / SR,
+                                                        ' (signal %d)' % idx[k])
+                kept[k] = self.apply_vad(xv, speech[k])
+            except Exception as e:
+                out[k] = e
+        x = [x for k in kept for _, _, x in kept[k]]
+        preds = self.gender_detection_mlp_model.predict(np.asarray(x, dtype=np.float32).reshape(len(x), EMBED_DIM))
+        pos = 0
+        for k, xv in kept.items():
+            gender_pred = preds[pos:pos + len(xv)]
+            pos += len(xv)
+            if len(gender_pred) > 1:
+                gender_pred = np.squeeze(gender_pred)
+            g = [(seg[0], seg[1], p) for (_, seg, _), p in zip(xv, gender_pred)]
+            try:
+                out[k] = (get_femininity_score(g), out[k][1], len(g))
+            except ZeroDivisionError as e:
+                out[k] = e
+        return out
 
     def __call__(self, fpath):
         """Voice femininity score of a media file (vbx_segmenter.py:147-202)."""

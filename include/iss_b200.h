@@ -39,7 +39,7 @@ typedef struct iss_mlp iss_mlp;
 
 /* ---- library / context ------------------------------------------------- */
 
-#define ISS_ABI_VERSION 3
+#define ISS_ABI_VERSION 4
 int         iss_version(void);               /* == ISS_ABI_VERSION of the header the library was built from */
 const char *iss_last_error(void);
 /* Creates a context bound to CUDA device `device` (one per host thread that
@@ -260,6 +260,16 @@ int64_t iss_vbx_work_bytes(int64_t n_samples);
  * no dither.  d_fea: float32 [M][64].  d_work: iss_vbx_work_bytes(n) of scratch. */
 int iss_vbx_features(iss_ctx *ctx, const void *d_pcm, int pcm_format, int64_t n_samples,
                      const double *d_dither, float *d_fea, void *d_work, void *stream);
+/* The same for n_rec recordings in one pair of launches (iss_vbx_features is its n_rec = 1 case).
+ * Recording r is h_pcm[r] (a DEVICE pointer held in a host array) with h_n_samples[r] samples, all
+ * in one pcm_format; its M_r = iss_vbx_num_frames(h_n_samples[r]) rows go to d_fea rows
+ * h_fea_off[r] .. + M_r.  Every recording is padded, dithered (d_dither[0 ..] again for each one,
+ * as the reference reseeds per get_features call), tiled and CMVN-windowed on its own, so its rows
+ * are bit-identical to those of an iss_vbx_features call on it.  Recordings under 200 samples get
+ * no rows.  d_work: 8 * 64 * sum(M_r) + 256 bytes of scratch. */
+int iss_vbx_features_multi(iss_ctx *ctx, int n_rec, const void *const *h_pcm, const int64_t *h_n_samples,
+                           int pcm_format, const double *d_dither, float *d_fea, const int64_t *h_fea_off,
+                           void *d_work, void *stream);
 
 /* ---- K5: ResNet101 x-vector extractor ----------------------------------------
  * Replaces VBxExtractor.get_embedding / OnnxBackendExtractor (vbx_segmenter.py:
