@@ -66,6 +66,7 @@ extern "C" int iss_ctx_create(int device, iss_ctx **out)
     c->recs_cap = 0;
     c->d_vbx_recs = nullptr;
     c->vbx_recs_cap = 0;
+    c->resample = nullptr;
     *out = c;
     return ISS_OK;
 }
@@ -78,6 +79,7 @@ extern "C" int iss_ctx_destroy(iss_ctx *ctx)
     if (ctx->d_partials) cudaFree(ctx->d_partials);
     if (ctx->d_recs) cudaFree(ctx->d_recs);
     if (ctx->d_vbx_recs) cudaFree(ctx->d_vbx_recs);
+    iss_resample_free(ctx);
     delete ctx;
     return ISS_OK;
 }

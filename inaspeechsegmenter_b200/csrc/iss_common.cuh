@@ -64,6 +64,10 @@ struct iss_ctx {
     int64_t recs_cap;            // in entries
     void *d_vbx_recs;            // per-recording table of a VBx features call (feat_vbx.cu)
     int64_t vbx_recs_cap;        // in entries
+    void *resample;              // tap tables and recording table of the resampler (resample.cu)
 };
+
+// Frees the resampler's device memory of a context (resample.cu).
+void iss_resample_free(iss_ctx *ctx);
 
 static inline cudaStream_t iss_stream(void *s) { return reinterpret_cast<cudaStream_t>(s); }

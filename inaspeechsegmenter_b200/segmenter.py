@@ -21,7 +21,7 @@ import warnings
 import numpy as np
 import torch
 
-from . import _lib, engine, models, pack
+from . import _lib, engine, models, pack, resample
 from .export_funcs import seg2csv, seg2textgrid
 from .io import media2sig16kmono
 from .sidekit_mfcc import SidekitFrontEnd
@@ -59,40 +59,51 @@ def _to_device_pcm(sig, device):
     return host.to(device, non_blocking=True)
 
 
-def _pass_input(sig):
+def _pass_input(sig, rate=16000):
     """A signal of segment_signals as a 1-D int16 / float32 numpy array or contiguous CUDA tensor (what
-    feats_from_signal would upload)."""
+    feats_from_signal would upload); a signal to resample (not 16 kHz mono) as resample.as_input returns it."""
+    if not resample.is_native(sig, rate):
+        return resample.as_input(sig)
     if isinstance(sig, torch.Tensor):
         if sig.is_cuda:
             if sig.dtype not in (torch.int16, torch.float32):
                 raise TypeError('pcm must be int16 or float32, got %s' % sig.dtype)
-            return sig.contiguous()
+            return sig.reshape(-1).contiguous()
         sig = sig.numpy()
-    sig = np.ascontiguousarray(sig)
+    sig = np.ascontiguousarray(sig).reshape(-1)
     if sig.dtype not in (np.int16, np.float32):
         sig = sig.astype(np.float32)
     return sig
 
 
-def _stage_pass(sigs, stage_off, dev):
-    """Device views of the signals of one pass (numpy arrays or CUDA tensors of one dtype): CUDA tensors are used in
-    place, host arrays are copied into one pinned staging buffer at stage_off (pack.PassLayout: each recording 16-byte
-    aligned) and uploaded in one copy."""
+_TORCH_DTYPE = {np.dtype(np.int16): torch.int16, np.dtype(np.float32): torch.float32}
+
+
+def _stage_pass(sigs, dev):
+    """Device views of the signals of one pass (numpy arrays or CUDA tensors, int16 or float32, any shape): CUDA
+    tensors are used in place, host arrays are copied into one pinned staging buffer, each 16-byte aligned (vector
+    loads in the kernels), and uploaded in one copy."""
     host = [i for i, s in enumerate(sigs) if isinstance(s, np.ndarray)]
     pcms = list(sigs)
     if host:
-        stage = np.zeros(int(stage_off[-1]), dtype=sigs[host[0]].dtype)
-        for i in host:
-            stage[stage_off[i]:stage_off[i] + sigs[i].shape[0]] = sigs[i]
+        off = np.concatenate(([0], np.cumsum([(sigs[i].nbytes + 15) // 16 * 16 for i in host]))).astype(np.int64)
+        stage = np.zeros(int(off[-1]), dtype=np.uint8)
+        for k, i in enumerate(host):
+            stage[off[k]:off[k] + sigs[i].nbytes] = sigs[i].reshape(-1).view(np.uint8)
         buf = torch.from_numpy(stage)
         try:
             buf = buf.pin_memory()
         except RuntimeError:
             pass
         buf = buf.to(dev, non_blocking=True)
-        for i in host:
-            pcms[i] = buf[stage_off[i]:stage_off[i] + sigs[i].shape[0]]
+        for k, i in enumerate(host):
+            pcms[i] = buf[off[k]:off[k] + sigs[i].nbytes].view(_TORCH_DTYPE[sigs[i].dtype]).view(sigs[i].shape)
     return pcms
+
+
+def _pass_pcms(ctx, sigs, rates):
+    """16 kHz mono device recordings of one pass: the signals staged at their own rate, then resampled per group."""
+    return resample.resample_pass(ctx, _stage_pass(sigs, ctx.device), rates)
 
 
 def feats_from_signal(sig, device=0, fft_precision=_lib.FFT_FP64, ctx_name='feat', medianame='<array>'):
@@ -308,38 +319,47 @@ class Segmenter:
             start_sec = 0
         return self.segment_feats(mspec, loge, difflen, start_sec)
 
-    def segment_signal(self, sig, start_sec=0):
-        """Extension: segment an in-memory 16 kHz mono signal (numpy int16/float32 or CUDA tensor)."""
+    def segment_signal(self, sig, start_sec=0, sample_rate=16000):
+        """Extension: segment an in-memory signal (numpy int16/float32 or CUDA tensor).  16 kHz mono ([frames]) goes to
+        the front end as it is; any other rate or channel count (``sample_rate`` an integer from 8000 to 192000 Hz,
+        int16 or float32 [frames, channels] with 1 to 8 channels) is first resampled to 16 kHz mono int16 on the device
+        (``resample``)."""
+        if not resample.is_native(sig, sample_rate):
+            sig = resample.to16k(self.ctx, sig, sample_rate)
+        elif len(resample.shape(sig)) == 2:
+            sig = sig.reshape(-1)
         mspec, loge, difflen = feats_from_signal(sig, self.device, self.fft_precision, 'main')
         return self.segment_feats(mspec, loge, difflen, start_sec)
 
-    def segment_signals(self, signals, start_secs=None):
-        """Extension: segment a list of in-memory 16 kHz mono signals (each what ``segment_signal`` accepts) in as few
-        device passes as possible.  Returns one segment list per signal, in input order, equal to
-        ``segment_signal(signals[i], start_secs[i])``.  Host arrays are staged in one pinned buffer per pass; CUDA
-        tensors are read in place.  Signals of 65536 frames (10.9 min) or more go through ``segment_signal``."""
+    def segment_signals(self, signals, start_secs=None, sample_rates=None):
+        """Extension: segment a list of in-memory signals (each what ``segment_signal`` accepts, at the rate
+        ``sample_rates[i]``, 16000 by default) in as few device passes as possible.  Returns one segment list per
+        signal, in input order, equal to ``segment_signal(signals[i], start_secs[i], sample_rates[i])``.  Host arrays
+        are staged in one pinned buffer per pass; CUDA tensors are read in place.  Signals are grouped and routed by
+        their 16 kHz length: those of 65536 frames (10.9 min) or more go through ``segment_signal``."""
         n = len(signals)
         if start_secs is None:
             start_secs = [0] * n
         if len(start_secs) != n:
             raise ValueError('%d signals but %d start times' % (n, len(start_secs)))
-        sigs = [_pass_input(s) for s in signals]
-        pack.check_lengths([s.shape[0] for s in sigs])
-        passes, long_ = pack.plan_passes([s.shape[0] for s in sigs], [str(s.dtype).split('.')[-1] for s in sigs])
+        rates = resample.check_rates(sample_rates, n)
+        sigs = [_pass_input(s, r) for s, r in zip(signals, rates)]
+        passes, long_ = resample.plan(sigs, rates)
         out = [None] * n
         for idx in passes:
-            for i, segs in zip(idx, self._segment_pass([sigs[i] for i in idx], [start_secs[i] for i in idx])):
+            for i, segs in zip(idx, self._segment_pass([sigs[i] for i in idx], [start_secs[i] for i in idx],
+                                                       [rates[i] for i in idx])):
                 out[i] = segs
         for i in long_:
-            out[i] = self.segment_signal(signals[i], start_secs[i])
+            out[i] = self.segment_signal(signals[i], start_secs[i], rates[i])
         return out
 
-    def _segment_pass(self, sigs, start_secs):
-        """One device pass over signals of one PCM format, each shorter than pack.LONG_FRAMES frames."""
+    def _segment_pass(self, sigs, start_secs, rates):
+        """One device pass over signals whose 16 kHz recordings share one PCM format, each shorter than
+        pack.LONG_FRAMES frames at 16 kHz."""
         dev = self.ctx.device
-        itemsize = sigs[0].itemsize if isinstance(sigs[0], np.ndarray) else sigs[0].element_size()
-        layout = pack.PassLayout([s.shape[0] for s in sigs], itemsize)
-        pcms = _stage_pass(sigs, layout.stage_off, dev)
+        pcms = _pass_pcms(self.ctx, sigs, rates)
+        layout = pack.PassLayout([p.shape[0] for p in pcms], pcms[0].element_size())
         mspec, loge, stats = _get_frontend('main', dev.index).multi(pcms, layout, self.fft_precision)
         for i in np.flatnonzero(layout.difflen > 0):
             # short media: pad with rows of min(mspec) (segmenter.py:60-65)

@@ -403,16 +403,25 @@ class VoiceFemininityScoring:
                 midpoint_seg.append((ratio, key, (start, stop), x))
         return add_needed_vectors(kept, midpoint_seg)
 
-    def score_signal(self, sig, basename='signal'):
-        """The body of __call__ on a decoded 16 kHz mono signal (numpy int16 / float)."""
-        sig = np.asarray(sig)
+    def score_signal(self, sig, basename='signal', sample_rate=16000):
+        """The body of __call__ on a decoded signal: 16 kHz mono numpy int16 / float, or, at any other ``sample_rate``
+        or channel count, what ``Segmenter.segment_signal`` resamples (then resampled to 16 kHz int16 on the device)."""
+        from . import resample
+        if not resample.is_native(sig, sample_rate):
+            sig = pcm = resample.to16k(self.ctx, sig, sample_rate)
+        else:
+            sig = np.asarray(sig)
+            sig = sig.reshape(-1) if sig.ndim == 2 else sig
+            sig = sig if sig.dtype in (np.int16, np.float32) else sig.astype(np.float32)
+            pcm = None
         duration = len(sig) / SR
-        vad_seg = self.vad.segment_signal(sig if sig.dtype in (np.int16, np.float32) else sig.astype(np.float32))
+        vad_seg = self.vad.segment_signal(sig)
         speech = [(b, e) for lab, b, e in vad_seg if lab == 'speech']
         speech_duration = sum(e - b for b, e in speech)
         if not speech_duration:
             return None, speech_duration, 0
-        pcm = torch.from_numpy(np.ascontiguousarray(sig if sig.dtype == np.int16 else sig.astype(np.float32))).to(self.ctx.device)
+        if pcm is None:
+            pcm = torch.from_numpy(np.ascontiguousarray(sig)).to(self.ctx.device)
         features = self.frontend(pcm)
         x_vectors = self.xvector_model(basename, features, duration)
         x_vectors = self.apply_vad(x_vectors, speech)
@@ -423,26 +432,31 @@ class VoiceFemininityScoring:
         g = [(seg[0], seg[1], p) for (_, seg, _), p in zip(x_vectors, gender_pred)]
         return get_femininity_score(g), speech_duration, len(g)
 
-    def score_signals(self, signals, basename='signal'):
+    def score_signals(self, signals, basename='signal', sample_rates=None):
         """score_signal on each of a list of signals (what score_signal takes, or 1-D int16 / float32 CUDA tensors, read in
-        place) in as few device passes as possible: one (score, speech_duration, nb_vectors) per signal, in input order,
-        equal to score_signal(signals[i]).  Per pass of pack.plan_passes, host arrays are staged and uploaded once, the VAD
-        runs as Segmenter.segment_signals, the VBx features of the recordings with speech as one K4 launch pair, their
-        x-vectors as one ResNet call for all regular windows plus one per tail length, and the MLP once.  Signals of
-        pack.LONG_FRAMES frames or more go through score_signal.  If score_signal would raise for some signals, the
-        exception of the first of them is raised."""
+        place, at the rate sample_rates[i], 16000 by default) in as few device passes as possible: one
+        (score, speech_duration, nb_vectors) per signal, in input order, equal to score_signal(signals[i], basename,
+        sample_rates[i]).  Per pass of pack.plan_passes over the 16 kHz lengths, host arrays are staged and uploaded
+        once, each (rate, channels, dtype) group is resampled in one launch, the VAD runs as Segmenter.segment_signals,
+        the VBx features of the recordings with speech as one K4 launch pair, their x-vectors as one ResNet call for all
+        regular windows plus one per tail length, and the MLP once.  Signals of pack.LONG_FRAMES frames or more at
+        16 kHz go through score_signal.  If score_signal would raise for some signals, the exception of the first of
+        them is raised."""
+        from . import resample
         from .segmenter import _pass_input
-        sigs = [_pass_input(s) for s in signals]
-        pack.check_lengths([s.shape[0] for s in sigs])
-        passes, long_ = pack.plan_passes([s.shape[0] for s in sigs], [str(s.dtype).split('.')[-1] for s in sigs])
+        rates = resample.check_rates(sample_rates, len(signals))
+        sigs = [_pass_input(s, r) for s, r in zip(signals, rates)]
+        passes, long_ = resample.plan(sigs, rates)
         out = [None] * len(sigs)
         for idx in passes:
-            for i, r in zip(idx, self._score_pass([sigs[i] for i in idx], idx, basename)):
+            for i, r in zip(idx, self._score_pass([sigs[i] for i in idx], idx, basename, [rates[i] for i in idx])):
                 out[i] = r
         for i in long_:
-            sig = signals[i].cpu().numpy() if isinstance(signals[i], torch.Tensor) else signals[i]
+            sig = signals[i]
+            if isinstance(sig, torch.Tensor) and resample.is_native(sig, rates[i]):
+                sig = sig.cpu().numpy()
             try:
-                out[i] = self.score_signal(sig, basename)
+                out[i] = self.score_signal(sig, basename, rates[i])
             except Exception as e:          # raised below, in input order
                 out[i] = e
         for r in out:
@@ -450,12 +464,11 @@ class VoiceFemininityScoring:
                 raise r
         return out
 
-    def _score_pass(self, sigs, idx, basename):
-        """One pass of score_signals over signals of one PCM format (idx: their input indices).  A recording for which
-        score_signal would raise gets the exception as its result."""
-        from .segmenter import _stage_pass
-        itemsize = sigs[0].itemsize if isinstance(sigs[0], np.ndarray) else sigs[0].element_size()
-        pcms = _stage_pass(sigs, pack.PassLayout([s.shape[0] for s in sigs], itemsize).stage_off, self.ctx.device)
+    def _score_pass(self, sigs, idx, basename, rates):
+        """One pass of score_signals over signals whose 16 kHz recordings share one PCM format (idx: their input
+        indices).  A recording for which score_signal would raise gets the exception as its result."""
+        from .segmenter import _pass_pcms
+        pcms = _pass_pcms(self.ctx, sigs, rates)
         speech = [[(b, e) for lab, b, e in segs if lab == 'speech'] for segs in self.vad.segment_signals(pcms)]
         out = [(None, sum(e - b for b, e in sp), 0) for sp in speech]
         live = [k for k, sp in enumerate(speech) if out[k][1]]

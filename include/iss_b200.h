@@ -39,7 +39,7 @@ typedef struct iss_mlp iss_mlp;
 
 /* ---- library / context ------------------------------------------------- */
 
-#define ISS_ABI_VERSION 4
+#define ISS_ABI_VERSION 5
 int         iss_version(void);               /* == ISS_ABI_VERSION of the header the library was built from */
 const char *iss_last_error(void);
 /* Creates a context bound to CUDA device `device` (one per host thread that
@@ -270,6 +270,36 @@ int iss_vbx_features(iss_ctx *ctx, const void *d_pcm, int pcm_format, int64_t n_
 int iss_vbx_features_multi(iss_ctx *ctx, int n_rec, const void *const *h_pcm, const int64_t *h_n_samples,
                            int pcm_format, const double *d_dither, float *d_fea, const int64_t *h_fea_off,
                            void *d_work, void *stream);
+
+/* ---- Resampling to 16 kHz mono -----------------------------------------------
+ * No reference counterpart: the reference has ffmpeg decode with `-ar 16000 -ac 1`
+ * (io.py:37-55).  This is NOT ffmpeg's resampler.  A recording of n frames of C
+ * interleaved channels at integer rate R (8000 <= R <= 192000, 1 <= C <= 8, int16 or
+ * float32 samples laid out [frames][channels]) becomes int16 16 kHz mono PCM:
+ *   x[m]   = mean of the C samples of frame m in float64 (int16 s as s / 32768.0),
+ *   y      = scipy.signal.resample_poly(x, up, down) with up = 16000 / g, down = R / g,
+ *            g = gcd(16000, R) (scipy's default Kaiser(5.0) design, zero padding),
+ *   out[k] = clip(rint(y[k] * 32768), -32768, 32767)  (round half to even),
+ * k < ceil(n * up / down).  Each output is one float64 dot product in a fixed tap
+ * order, so every recording's output is the same in any call. */
+
+/* ceil(n_frames * up / down); -1 for a rate outside [8000, 192000] or n_frames < 0. */
+int64_t iss_resample_num_frames(int64_t n_frames, int rate);
+/* h_taps: the float64 prototype filter of rate `rate`, scipy.signal.firwin(2H + 1,
+ * 1 / max(up, down), window=('kaiser', 5.0)) * up with H = 10 max(up, down) (n_taps =
+ * 2H + 1; the single tap {1.0} when up == down == 1).  Arranged by phase and kept on
+ * the device by the context until iss_resample_release_taps or iss_ctx_destroy; an
+ * upload for a rate that has taps replaces them.  Synchronous. */
+int iss_resample_upload_taps(iss_ctx *ctx, int rate, const double *h_taps, int64_t n_taps);
+int iss_resample_release_taps(iss_ctx *ctx, int rate);
+/* Resamples n_rec recordings of one (rate, channels, pcm_format) in one launch.  Recording
+ * r is h_pcm[r] (a DEVICE pointer held in a host array) with h_n_frames[r] frames; its
+ * iss_resample_num_frames(h_n_frames[r], rate) int16 outputs go to d_out[h_out_off[r] ..].
+ * Any pointer alignment of the sample type works (16-byte aligned recordings are read
+ * with vector loads).  ISS_ERR_STATE if no taps were uploaded for `rate`. */
+int iss_resample_to16k_multi(iss_ctx *ctx, int n_rec, const void *const *h_pcm, const int64_t *h_n_frames,
+                             int channels, int rate, int pcm_format, int16_t *d_out, const int64_t *h_out_off,
+                             void *stream);
 
 /* ---- K5: ResNet101 x-vector extractor ----------------------------------------
  * Replaces VBxExtractor.get_embedding / OnnxBackendExtractor (vbx_segmenter.py:
