@@ -92,6 +92,8 @@ SIGNATURES = {
     'iss_cnn_profile_read': (_i, [_vp, _c.POINTER(_d), _c.POINTER(_i64), _c.POINTER(_d)]),
     'iss_cnn_layer_flops': (_d, [_vp, _i]),
     'iss_cnn_num_layers': (_i, [_vp]),
+    'iss_gather_halo_rows_bound': (_i, [_i, _i, _i, _i, _i, _i]),
+    'iss_gather_halo_smem': (_i, [_i] * 10),
 }
 
 

@@ -39,6 +39,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
 #include <vector>
 
 #include "conv_gemm.cuh"
@@ -51,6 +52,11 @@ constexpr int TBM = 128, TBK = 32, HBK = 64;
 constexpr int THREADS = 256;
 constexpr int A_WG = 16384;                  // one warpgroup's operand tile of one stage: hi | lo, 64 rows x 128 B each
 constexpr int A_STAGES = 2, B_STAGES = 4;
+constexpr int MAX_SMEM = 227 * 1024;
+// Tile halo of the pooled fill (LD_POOL) of 64 channels and more than one tap: every pooled input pixel the tile's output
+// rows read, one word per channel.  The weight ring shrinks to three stages, one k-block ahead, to make room for it.
+constexpr int HALO_PIX = 64 * 4;
+constexpr int HALO_B_STAGES = 3;
 
 constexpr int ENG_TF32 = 0, ENG_F16 = 1;
 // operand fill of engine 3: fp32 values split here, split-half words, words with the 2x2 max-pooling in front (gather
@@ -62,6 +68,33 @@ struct WgCfg {
     static constexpr int B_STAGE = 2 * BN * 128;                         // hi | lo, BN rows x 128 B each
     static constexpr int SMEM = B_STAGES * B_STAGE + A_STAGES * 2 * A_WG + 1024;
 };
+
+// shared memory of the gather kernel with a halo of `rows` input rows of width W
+int halo_smem(int BN, int rows, int W)
+{
+    return HALO_B_STAGES * 2 * BN * 128 + A_STAGES * 2 * A_WG + 1024 + rows * W * HALO_PIX;
+}
+
+// 2x2 window maximum of split-half words at the four window offsets `offs` (words of `in`): the WORD of the largest value
+// is kept, as maxpool_nhwc_kernel<uint4> does: window order (0,0) (0,1) (1,0) (1,1), NaN wins, first maximum wins
+template <int NW>
+__device__ __forceinline__ void pool_max_words(const uint32_t *in, const int64_t (&offs)[4], uint32_t (&bw)[NW])
+{
+    float bv[NW];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+#pragma unroll
+        for (int h = 0; h < NW / 4; ++h) {
+            const uint4 u = __ldg(reinterpret_cast<const uint4 *>(in + offs[q]) + h);
+            const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const float fv = iss_unpack_split(w[e]);
+                if (q == 0 || fv > bv[4 * h + e] || fv != fv) { bv[4 * h + e] = fv; bw[4 * h + e] = w[e]; }
+            }
+        }
+    }
+}
 
 __device__ __forceinline__ void split_f16(const float (&v)[8], uint32_t (&hw)[4], uint32_t (&lw)[4])
 {
@@ -150,19 +183,25 @@ __device__ __forceinline__ void epi_store1(const ConvArgs &a, const EpiCoef1 &c,
     else *dst = v;
 }
 
+// halo_rows > 0 (LD_POOL with C = 64 only): the tile's pooled input rows fit in a halo of that many rows.  The tile then
+// takes the 2x2 maximum of each of them once, stages the words in shared memory and fills every tap from there instead of
+// taking the maximum of four global words per tap and value.
 template <int ENG, int BN, int MODE>
 __global__ void __launch_bounds__(THREADS, 1)
-conv_gemm_wg_kernel(const ConvArgs a, const unsigned char *__restrict__ wt, float inv_scale)
+conv_gemm_wg_kernel(const ConvArgs a, const unsigned char *__restrict__ wt, float inv_scale, int halo_rows)
 {
     using Cfg = WgCfg<BN>;
     constexpr int KE = ENG == ENG_F16 ? HBK : TBK;                       // k-elements per block
     constexpr int RAW = ENG == ENG_F16 ? 2 : 1;                          // 16-byte input loads per 16-byte operand chunk
     constexpr bool PREFETCH = MODE == LD_F32 || MODE == LD_PACKED;       // raw input held in registers one k-block ahead
+    const bool halo = MODE == LD_POOL && halo_rows > 0;
+    const int b_stages = halo ? HALO_B_STAGES : B_STAGES, b_ahead = b_stages - 2;
     extern __shared__ unsigned char smem_dyn[];
     unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
     unsigned char *b_ring = smem;
     const uint32_t b_ring_u32 = smem_u32(b_ring);
-    const uint32_t a_ring_u32 = b_ring_u32 + B_STAGES * Cfg::B_STAGE;
+    const uint32_t a_ring_u32 = b_ring_u32 + (uint32_t)b_stages * Cfg::B_STAGE;
+    const uint32_t halo_u32 = a_ring_u32 + A_STAGES * 2 * A_WG;
 
     const int tid = threadIdx.x, wg = tid >> 7, t = tid & 127;
     const int64_t m0 = (int64_t)blockIdx.x * TBM + wg * 64;
@@ -173,14 +212,13 @@ conv_gemm_wg_kernel(const ConvArgs a, const unsigned char *__restrict__ wt, floa
     auto issue_b = [&](int kb) {
         if (kb < nkb) {
             const unsigned char *src = wtile + (size_t)kb * Cfg::B_STAGE;
-            const uint32_t dst = b_ring_u32 + (uint32_t)(kb % B_STAGES) * Cfg::B_STAGE;
+            const uint32_t dst = b_ring_u32 + (uint32_t)(kb % b_stages) * Cfg::B_STAGE;
 #pragma unroll
             for (int o = tid * 16; o < Cfg::B_STAGE; o += THREADS * 16) cp_async16_u32(dst + o, src + o, 16);
         }
         cp_async_commit();                                   // (empty groups keep the group count uniform)
     };
-    issue_b(0);
-    issue_b(1);
+    for (int kb = 0; kb < b_ahead; ++kb) issue_b(kb);
 
     // this thread's operand rows (64 per warpgroup): r_i = t / 8 + 16 i, 16-byte chunk j of the 128-byte operand row
     const int j = t & 7;
@@ -201,6 +239,39 @@ conv_gemm_wg_kernel(const ConvArgs a, const unsigned char *__restrict__ wt, floa
         row_iw0[i] = ow * a.SW - a.PL;
     }
     const uint32_t row_dst0 = (uint32_t)((t >> 3) * 128 + ((j ^ ((t >> 3) & 7)) << 4));   // (t/8 + 16 i) & 7 == (t/8) & 7
+    // The halo holds the pixels of the rows g_lo .. g_lo + halo_n - 1 of the batch as one tall image (row img * H + ih):
+    // from the first input row of the tile's first output row to the last input row of its last one.  Row i's pixel
+    // (ih, iw) is halo pixel (row_hb[i] + ih) * W + iw.
+    int64_t g_lo = 0;
+    int halo_n = 0, row_hb[4];
+    if (halo) {
+        const int64_t ohw = (int64_t)a.OH * a.OW;
+        const int64_t mf = (int64_t)blockIdx.x * TBM, ml = (mf + TBM < a.M ? mf + TBM : a.M) - 1;
+        const int64_t img0 = mf / ohw, img1 = ml / ohw;
+        const int oh0 = (int)(mf - img0 * ohw) / a.OW, oh1 = (int)(ml - img1 * ohw) / a.OW;
+        g_lo = img0 * a.H + max(oh0 * a.SH - a.PT, 0);
+        halo_n = (int)(img1 * a.H + min(oh1 * a.SH - a.PT + a.KH - 1, a.H - 1) - g_lo + 1);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) row_hb[i] = (int)((int64_t)row_img[i] * a.H - g_lo);
+    }
+    if constexpr (MODE == LD_POOL) {
+        if (halo) {                                          // stage the halo: 16 chunks of 16 bytes per pixel
+            const int nu = halo_n * a.W * 16;
+#pragma unroll 4
+            for (int u = tid; u < nu; u += THREADS) {
+                const int px = u >> 4, q = u & 15;
+                const int64_t gp = g_lo * a.W + px;          // pixel of the tall pooled image
+                const int64_t gr = gp / a.W, img = gr / a.H;
+                const int iw = (int)(gp - gr * a.W), ih = (int)(gr - img * a.H);
+                const int64_t p00 = ((img * a.pool_h + 2 * ih) * a.pool_w + 2 * iw) * a.C + q * 4;
+                const int64_t offs[4] = {p00, p00 + a.C, p00 + (int64_t)a.pool_w * a.C, p00 + (int64_t)a.pool_w * a.C + a.C};
+                uint32_t w[4];
+                pool_max_words(reinterpret_cast<const uint32_t *>(a.in), offs, w);
+                sts128(halo_u32 + (uint32_t)u * 16u, w[0], w[1], w[2], w[3]);
+            }
+            __syncthreads();
+        }
+    }
     // tap of the next k-block to fill: k = (rr * KW + ss) * C + c0
     int tap_c0 = 0, tap_ss = 0, tap_rr = 0;
     auto advance = [&]() {
@@ -257,22 +328,18 @@ conv_gemm_wg_kernel(const ConvArgs a, const unsigned char *__restrict__ wt, floa
                 // (as maxpool_nhwc_kernel<uint4> does: window order (0,0) (0,1) (1,0) (1,1), NaN wins, first maximum wins)
                 uint32_t bw[8] = {0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
                 int ih, iw;
-                if (pixel_ok(i, ih, iw)) {
-                    const uint32_t *in = reinterpret_cast<const uint32_t *>(a.in);
+                if (pixel_ok(i, ih, iw) && halo) {
+                    // the 8 words of chunk j from the halo; threads j >= 4 read their two 16-byte halves in the other
+                    // order, so that the 8 chunks of a quarter warp hit all 32 banks
+                    const uint32_t p = halo_u32 + (uint32_t)((row_hb[i] + ih) * a.W + iw) * HALO_PIX + j * 32;
+                    const uint32_t sw = (uint32_t)(j & 4) << 2;
+                    const uint4 x = lds128(p + sw), y = lds128(p + (sw ^ 16u));
+                    const uint4 u0 = sw ? y : x, u1 = sw ? x : y;
+                    bw[0] = u0.x; bw[1] = u0.y; bw[2] = u0.z; bw[3] = u0.w; bw[4] = u1.x; bw[5] = u1.y; bw[6] = u1.z; bw[7] = u1.w;
+                } else if (pixel_ok(i, ih, iw)) {
                     const int64_t p00 = (((int64_t)row_img[i] * a.pool_h + 2 * ih) * a.pool_w + 2 * iw) * a.C + tap_c0 + j * 8;
                     const int64_t offs[4] = {p00, p00 + a.C, p00 + (int64_t)a.pool_w * a.C, p00 + (int64_t)a.pool_w * a.C + a.C};
-                    float bv[8];
-#pragma unroll
-                    for (int q = 0; q < 4; ++q) {
-                        const uint4 u0 = __ldg(reinterpret_cast<const uint4 *>(in + offs[q]));
-                        const uint4 u1 = __ldg(reinterpret_cast<const uint4 *>(in + offs[q]) + 1);
-                        const uint32_t w[8] = {u0.x, u0.y, u0.z, u0.w, u1.x, u1.y, u1.z, u1.w};
-#pragma unroll
-                        for (int e = 0; e < 8; ++e) {
-                            const float fv = iss_unpack_split(w[e]);
-                            if (q == 0 || fv > bv[e] || fv != fv) { bv[e] = fv; bw[e] = w[e]; }
-                        }
-                    }
+                    pool_max_words(reinterpret_cast<const uint32_t *>(a.in), offs, bw);
                 }
                 words_to_planes(bw, hw, lw);
             }
@@ -291,14 +358,15 @@ conv_gemm_wg_kernel(const ConvArgs a, const unsigned char *__restrict__ wt, floa
         const int s = kb & 1;
         fill(s);                                             // stage s was last read by this warpgroup's wgmmas of kb - 2
         if constexpr (PREFETCH) { if (kb + 1 < nkb) fetch(); }
-        cp_async_wait<1>();                                  // weights of kb landed (kb + 1 may still be in flight)
+        if (halo) cp_async_wait<0>();                        // weights of kb landed
+        else cp_async_wait<1>();                             // (kb + 1 may still be in flight)
         fence_proxy_async();
         __syncthreads();
-        issue_b(kb + 2);                                     // its stage was read by kb - 2, retired in every warpgroup
+        issue_b(kb + b_ahead);                               // its stage was read by kb - 2, retired in every warpgroup
         wgmma_fence();
         const uint64_t da = make_sw128_desc(a_ring_u32 + (uint32_t)(s * 2 + wg) * A_WG);
         const uint64_t dal = da + ((A_WG / 2) >> 4);
-        const uint64_t db = make_sw128_desc(b_ring_u32 + (uint32_t)(kb % B_STAGES) * Cfg::B_STAGE);
+        const uint64_t db = make_sw128_desc(b_ring_u32 + (uint32_t)(kb % b_stages) * Cfg::B_STAGE);
         const uint64_t dbl = db + ((BN * 128) >> 4);
 #pragma unroll
         for (int kk = 0; kk < 4; ++kk) {                     // 32 bytes of the operand row per wgmma (k16 fp16 / k8 tf32)
@@ -339,11 +407,13 @@ int launch_wg(const ConvArgs &a, const void *wt, float inv_scale, cudaStream_t s
 {
     using Cfg = WgCfg<BN>;
     auto kern = conv_gemm_wg_kernel<ENG, BN, MODE>;
-    ISS_CUDA_OK(iss_optin_smem(reinterpret_cast<const void *>(kern), Cfg::SMEM));
+    const int halo_rows = MODE == LD_POOL ? iss_gather_halo_rows(a) : 0;
+    const int smem = halo_rows > 0 ? halo_smem(BN, halo_rows, a.W) : Cfg::SMEM;
+    ISS_CUDA_OK(iss_optin_smem(reinterpret_cast<const void *>(kern), smem));
     const int64_t gm = (a.M + TBM - 1) / TBM;
     ISS_REQUIRE(gm < (1ll << 31), ISS_ERR_INVALID, "conv_tc: M too large");
     dim3 grid((unsigned)gm, (unsigned)(a.N / BN));
-    kern<<<grid, THREADS, Cfg::SMEM, st>>>(a, reinterpret_cast<const unsigned char *>(wt), inv_scale);
+    kern<<<grid, THREADS, smem, st>>>(a, reinterpret_cast<const unsigned char *>(wt), inv_scale, halo_rows);
     ISS_CUDA_OK(cudaGetLastError());
     iss_count_launch();
     return ISS_OK;
@@ -383,7 +453,7 @@ constexpr int SLAB_PRODUCER_REGS = 56, SLAB_CONSUMER_REGS = 224;
 constexpr int SLAB_B_STAGE = 2 * SLAB_N * 128;          // hi | lo, 64 rows x 128 B each
 constexpr int SLAB_MAX_STAGES = 4, SLAB_MAX_BUF = 2;
 constexpr int SLAB_BAR_BYTES = 8 * 2 * (SLAB_MAX_STAGES + SLAB_MAX_BUF);
-constexpr int SLAB_MAX_SMEM = 227 * 1024;
+constexpr int SLAB_MAX_SMEM = MAX_SMEM;
 
 // slab rows of a tile (a multiple of 8, so that the lo plane stays 1024-byte aligned) and the kernel's shared memory:
 // `stages` weight stages, `nbuf` slabs and 1024 bytes of alignment slack, which also hold the mbarriers
@@ -635,6 +705,38 @@ int upload(const void *h, size_t bytes, void **d_out, const char *what)
 int g_gemm_mode = -1;      // -1 = read ISS_B200_GEMM on first use
 
 }  // namespace
+
+// Input rows (of the batch as one tall image, row img * H + ih) that the 128 output rows of one tile read, at most over
+// every tile start: tiles start at multiples of 128, i.e. at the positions s * gcd(128, OH * OW) of an image.
+extern "C" int iss_gather_halo_rows_bound(int H, int OH, int OW, int KH, int SH, int PT)
+{
+    const int64_t ohw = (int64_t)OH * OW;
+    int64_t g = TBM, r = ohw;
+    while (r) { const int64_t q = g % r; g = r; r = q; }
+    int64_t rows = 0;
+    for (int64_t s = 0; s < ohw; s += g) {
+        const int64_t last = s + TBM - 1, img1 = last / ohw;
+        const int64_t oh0 = s / OW, oh1 = (last - img1 * ohw) / OW;
+        const int64_t lo = std::max<int64_t>(oh0 * SH - PT, 0), hi = img1 * H + std::min<int64_t>(oh1 * SH - PT + KH - 1, H - 1);
+        rows = std::max(rows, hi - lo + 1);
+    }
+    return (int)rows;
+}
+
+// Shared memory of a gather-kernel layer with the pooling folded in (LD_POOL) when it takes the halo, 0 for the
+// global-memory fill: the halo holds one 64-channel block (C = 64), filters with one tap reuse no input, and the halo
+// must fit in shared memory next to the rings.
+extern "C" int iss_gather_halo_smem(int H, int W, int OH, int OW, int KH, int KW, int SH, int PT, int C, int N)
+{
+    if (C != HBK || KH * KW == 1) return 0;
+    const int smem = halo_smem(f16_bn_for(N), iss_gather_halo_rows_bound(H, OH, OW, KH, SH, PT), W);
+    return smem <= MAX_SMEM ? smem : 0;
+}
+
+int iss_gather_halo_rows(const ConvArgs &a)
+{
+    return iss_gather_halo_smem(a.H, a.W, a.OH, a.OW, a.KH, a.KW, a.SH, a.PT, a.C, a.N) ? iss_gather_halo_rows_bound(a.H, a.OH, a.OW, a.KH, a.SH, a.PT) : 0;
+}
 
 // Does the slab kernel take this engine-3 layer?  Un-padded, stride-1 'valid' convolution, 64 -> 64 channels, no
 // folded pooling, and one slab plus a four-stage weight ring fit in shared memory.

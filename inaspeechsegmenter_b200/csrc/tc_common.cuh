@@ -56,6 +56,12 @@ __device__ __forceinline__ void sts128(uint32_t addr, uint32_t x, uint32_t y, ui
 {
     asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(x), "r"(y), "r"(z), "r"(w) : "memory");
 }
+__device__ __forceinline__ uint4 lds128(uint32_t addr)
+{
+    uint4 v;
+    asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
+    return v;
+}
 
 // K-major, SWIZZLE_128B operand tile (rows of 128 bytes, 16-byte chunk j of row r stored at chunk j ^ (r & 7), 8-row
 // groups 1024 bytes apart, tile 1024-byte aligned).  Advancing K by 32 bytes inside the row adds 2 to the start address.

@@ -344,6 +344,16 @@ int iss_cnn_profile_read(iss_cnn *cnn, double *total_ms, int64_t *launches, doub
 /* FLOPs of one layer for one patch (2 * MACs); 0 for pooling. */
 double iss_cnn_layer_flops(const iss_cnn *cnn, int layer);
 int iss_cnn_num_layers(const iss_cnn *cnn);
+/* Input rows that one 128-row tile of the gather convolution kernel reads at most
+ * (rows of the batch as one tall image), over every tile start: the size of
+ * its shared-memory halo for a layer of input height H, output OH x OW, KH
+ * filter rows, row stride SH and top padding PT. */
+int iss_gather_halo_rows_bound(int H, int OH, int OW, int KH, int SH, int PT);
+/* Shared memory (bytes) of the gather convolution kernel with that halo for an
+ * fp16-split layer with a 2x2 max-pooling folded in, C -> N channels, pooled
+ * input width W and a KH x KW filter; 0 when the layer keeps the global-memory
+ * operand fill (C != 64, one tap, or the halo does not fit in shared memory). */
+int iss_gather_halo_smem(int H, int W, int OH, int OW, int KH, int KW, int SH, int PT, int C, int N);
 
 #ifdef __cplusplus
 }
