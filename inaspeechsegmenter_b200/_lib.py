@@ -94,6 +94,7 @@ SIGNATURES = {
     'iss_cnn_num_layers': (_i, [_vp]),
     'iss_gather_halo_rows_bound': (_i, [_i, _i, _i, _i, _i, _i]),
     'iss_gather_halo_smem': (_i, [_i] * 10),
+    'iss_gather_pipe_smem': (_i, [_i] * 10),
 }
 
 

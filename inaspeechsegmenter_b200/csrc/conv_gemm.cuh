@@ -159,6 +159,8 @@ IssConvKernel iss_conv_kernel(const ConvArgs &a, int mode);
 bool iss_slab_covers(const ConvArgs &a);
 // rows of the gather kernel's shared-memory halo for a layer with the pooling folded in (0: global-memory fill)
 int iss_gather_halo_rows(const ConvArgs &a);
+// the same rows when the layer takes the pipelined path with two halos (0: it keeps another path)
+int iss_gather_pipe_rows(const ConvArgs &a);
 int iss_launch_conv_tf32(const ConvArgs &a, cudaStream_t st);
 int iss_launch_conv_f16(const ConvArgs &a, cudaStream_t st);
 int iss_launch_conv_slab(const ConvArgs &a, cudaStream_t st);

@@ -28,7 +28,9 @@
 // issues its wgmmas.  The weights are static, so the host stores them already tiled and swizzled exactly as the shared
 // memory operand image ([n-tile][k-block][hi|lo][BN rows x 128 B]); all 256 threads copy a stage with cp.async, four
 // stages deep (two k-blocks ahead).  The global loads of k-block kb+1 are in flight while the wgmmas of kb are issued,
-// and wgmma.wait_group 1 keeps one k-block of tensor work running while the next tile is filled.
+// and wgmma.wait_group 1 keeps one k-block of tensor work running while the next tile is filled.  The pooled instance
+// (LD_POOL) launches 384 threads: where two tile halos fit it runs the persistent, warp-specialized gather_pipe, whose
+// A operands come from the halo through ldmatrix into registers; elsewhere its warpgroups 1 and 2 run the loop above.
 //
 // The un-padded, stride-1 64 -> 64 convolutions of engine 3 (the segmenter CNNs' dominant 5x4 layer, with or without the
 // fused first layer) run in conv_slab_kernel instead: it fills each input value once per tile into a "slab" whose
@@ -75,8 +77,69 @@ int halo_smem(int BN, int rows, int W)
     return HALO_B_STAGES * 2 * BN * 128 + A_STAGES * 2 * A_WG + 1024 + rows * W * HALO_PIX;
 }
 
-// 2x2 window maximum of split-half words at the four window offsets `offs` (words of `in`): the WORD of the largest value
-// is kept, as maxpool_nhwc_kernel<uint4> does: window order (0,0) (0,1) (1,0) (1,1), NaN wins, first maximum wins
+// Every launch of the pooled instance (LD_POOL) has 384 threads: on the pipelined path (gather_pipe) warpgroup 0 produces
+// and warpgroups 1 and 2 consume; on the other paths warpgroup 0 gives its registers away and exits, and warpgroups 1 and
+// 2 run the fill / wgmma loop of the other instances.
+constexpr int POOL_THREADS = 384;
+// the launch gives every thread 168 registers (384 threads, one CTA per SM): 128 x 24 + 256 x 240 = 128 x 112 + 256 x
+// 192 = 384 x 168, so that setmaxnreg.inc finds the registers that setmaxnreg.dec released
+constexpr int POOL_IDLE_REGS = 24, POOL_WG_REGS = 240;
+constexpr int PIPE_PRODUCER_REGS = 112, PIPE_CONSUMER_REGS = 192;
+constexpr int PIPE_FILL_THREADS = 96;                   // producer warps 1..3
+constexpr int PIPE_CONSUMER_ARRIVALS = 8;               // lane 0 of each consumer warp
+constexpr int PIPE_B_STAGES = 3, PIPE_HALOS = 2;
+constexpr int PIPE_BAR_BYTES = 8 * 2 * (PIPE_B_STAGES + PIPE_HALOS);
+
+// one halo buffer of the pipelined path: a hi plane and a lo plane of 128 bytes per pixel, for `rows` x W pixels and
+// one zero pixel (the operand rows of padding and of rows past M point at it)
+int pipe_halo_bytes(int rows, int W) { return 2 * (rows * W + 1) * 128; }
+// its shared memory: the weight ring, two halo buffers, and 1024 bytes of alignment slack that also hold the mbarriers
+int pipe_smem(int BN, int rows, int W) { return PIPE_B_STAGES * 2 * BN * 128 + PIPE_HALOS * pipe_halo_bytes(rows, W) + 1024; }
+
+// The rows of a 128-row tile's halo: the rows g_lo .. g_lo + n - 1 of the batch as one tall pooled image (row img * H +
+// ih), from the first input row of the tile's first output row to the last input row of its last one.
+__device__ __forceinline__ void halo_span(const ConvArgs &a, int64_t tile, int64_t &g_lo, int &n)
+{
+    const int64_t ohw = (int64_t)a.OH * a.OW;
+    const int64_t mf = tile * TBM, ml = (mf + TBM < a.M ? mf + TBM : a.M) - 1;
+    const int64_t img0 = mf / ohw, img1 = ml / ohw;
+    const int oh0 = (int)(mf - img0 * ohw) / a.OW, oh1 = (int)(ml - img1 * ohw) / a.OW;
+    g_lo = img0 * a.H + max(oh0 * a.SH - a.PT, 0);
+    n = (int)(img1 * a.H + min(oh1 * a.SH - a.PT + a.KH - 1, a.H - 1) - g_lo + 1);
+}
+
+// the four 2x2-window words of NW channels at the window offsets `offs` (words of `in`)
+template <int NW>
+__device__ __forceinline__ void pool_load(const uint32_t *in, const int64_t (&offs)[4], uint4 (&raw)[4][NW / 4])
+{
+#pragma unroll
+    for (int q = 0; q < 4; ++q)
+#pragma unroll
+        for (int h = 0; h < NW / 4; ++h) raw[q][h] = __ldg(reinterpret_cast<const uint4 *>(in + offs[q]) + h);
+}
+
+// 2x2 window maximum of split-half words: the WORD of the largest value is kept, as maxpool_nhwc_kernel<uint4> does:
+// window order (0,0) (0,1) (1,0) (1,1), NaN wins, first maximum wins
+template <int NW>
+__device__ __forceinline__ void pool_select(const uint4 (&raw)[4][NW / 4], uint32_t (&bw)[NW])
+{
+    float bv[NW];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+#pragma unroll
+        for (int h = 0; h < NW / 4; ++h) {
+            const uint4 u = raw[q][h];
+            const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const float fv = iss_unpack_split(w[e]);
+                if (q == 0 || fv > bv[4 * h + e] || fv != fv) { bv[4 * h + e] = fv; bw[4 * h + e] = w[e]; }
+            }
+        }
+    }
+}
+
+// the same maximum of the words at the four window offsets `offs` (words of `in`), loaded and selected in one pass
 template <int NW>
 __device__ __forceinline__ void pool_max_words(const uint32_t *in, const int64_t (&offs)[4], uint32_t (&bw)[NW])
 {
@@ -183,17 +246,218 @@ __device__ __forceinline__ void epi_store1(const ConvArgs &a, const EpiCoef1 &c,
     else *dst = v;
 }
 
+// epilogue of one warpgroup's 64 rows m0 .. m0 + 63 (thread t of the warpgroup) from its accumulators: hh + (hl + lh)
+template <int ENG, int BN>
+__device__ __forceinline__ void wg_epilogue(const ConvArgs &a, const float (&dm)[BN / 2], const float (&dl)[BN / 2], int64_t m0,
+                                            int n0, int t, float inv_scale)
+{
+    const int w = t >> 5, l = t & 31;
+    const int64_t mr = m0 + 16 * w + (l >> 2);
+#pragma unroll
+    for (int i = 0; i < BN / 8; ++i) {
+        const int nb = n0 + 8 * i + 2 * (l & 3);
+        const EpiCoef c = epi_coef(a, nb);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int64_t m = mr + 8 * h;
+            if (m >= a.M) continue;
+            epi_store<ENG>(a, c, m, nb, dm[4 * i + 2 * h] + dl[4 * i + 2 * h], dm[4 * i + 2 * h + 1] + dl[4 * i + 2 * h + 1], inv_scale);
+        }
+    }
+}
+
+// ============================ pipelined pooled path (LD_POOL, C = 64, two halos fit) ============================
+// Persistent: CTA i takes the 128-row tiles i, i + gridDim.x, ... in increasing order (so CTAs running at the same time
+// share input rows in L2).  Warpgroup 0 produces: its warp 0 streams the weight stage of every k-block (one tap of 64
+// channels) with one bulk copy into a three-stage ring, its warps 1..3 stage the halo of the next tile into the other of
+// two halo buffers.  A halo buffer holds the pooled pixel p of the tile's rows (halo_span) as a hi plane and a lo plane
+// of 128 bytes each, 16-byte chunk q (channels 8 q .. 8 q + 7) at chunk q ^ (p & 7), so that 8 consecutive pixels hit all
+// 32 banks.  Warpgroups 1 and 2 consume 64 output rows each: per k16 step each warp gathers its 16 im2col rows from the
+// halo with one ldmatrix.x4 for hi and one for lo (lane l gives row (l & 7) + 8 ((l >> 3) & 1), chunk 2 kk + l / 16)
+// and issues Ah.Bh, Ah.Bl and Al.Bh with A in registers: the same products in the same order as the other paths, into
+// the same two accumulators.  Full / empty mbarriers hand every weight stage and every halo buffer over.
+template <int BN>
+__device__ __forceinline__ void gather_pipe(const ConvArgs &a, const unsigned char *__restrict__ wt, float inv_scale, int halo_rows)
+{
+    constexpr int B_STAGE = WgCfg<BN>::B_STAGE;
+    extern __shared__ unsigned char smem_dyn[];
+    const uint32_t base = smem_u32(smem_dyn);
+    const uint32_t ring = (base + 1023u) & ~1023u;
+    const uint32_t halo0 = ring + (uint32_t)PIPE_B_STAGES * B_STAGE;
+    const int zp = halo_rows * a.W;                                     // the zero pixel
+    const uint32_t plane = (uint32_t)(zp + 1) * 128u, halo_bytes = 2 * plane;
+    const uint32_t bars = ring - base >= (uint32_t)PIPE_BAR_BYTES ? base : halo0 + PIPE_HALOS * halo_bytes;
+    const uint32_t wfull = bars, wempty = bars + 8 * PIPE_B_STAGES;                       // + 8 * stage
+    const uint32_t hfull = bars + 16 * PIPE_B_STAGES, hempty = hfull + 8 * PIPE_HALOS;     // + 8 * buffer
+
+    const int tid = threadIdx.x, wg = tid >> 7;
+    if (tid == 0) {
+        for (int s = 0; s < PIPE_B_STAGES; ++s) { mbar_init(wfull + 8 * s, 1); mbar_init(wempty + 8 * s, PIPE_CONSUMER_ARRIVALS); }
+        for (int b = 0; b < PIPE_HALOS; ++b) { mbar_init(hfull + 8 * b, PIPE_FILL_THREADS); mbar_init(hempty + 8 * b, PIPE_CONSUMER_ARRIVALS); }
+        fence_mbar_init();
+    }
+    if (tid < 2 * PIPE_HALOS * 8) {                                     // the zero pixel of both planes of both buffers
+        const int q = tid & 7, pl = tid >> 3;
+        sts128(halo0 + (uint32_t)(pl >> 1) * halo_bytes + (uint32_t)(pl & 1) * plane + (uint32_t)zp * 128u + q * 16, 0u, 0u, 0u, 0u);
+    }
+    __syncthreads();
+
+    const int nkb = a.KH * a.KW;                                        // one k-block (64 channels) per tap
+    const int64_t tiles = (a.M + TBM - 1) / TBM;
+    const unsigned char *wtile = wt + (size_t)blockIdx.y * nkb * B_STAGE;
+
+    if (wg == 0) {
+        // ============================ producer ============================
+        setmaxnreg_dec<PIPE_PRODUCER_REGS>();
+        if (tid < 32) {                                                 // warp 0: the weight stage of every k-block
+            if (tid == 0) {
+                int s = 0;
+                uint32_t ph = 0;
+                for (int64_t tile = blockIdx.x; tile < tiles; tile += gridDim.x)
+                    for (int kb = 0; kb < nkb; ++kb) {
+                        mbar_wait(wempty + 8 * s, ph ^ 1);              // both consumers retired the wgmmas that read it
+                        mbar_arrive_expect_tx(wfull + 8 * s, B_STAGE);
+                        bulk_copy_g2s(ring + (uint32_t)s * B_STAGE, wtile + (size_t)kb * B_STAGE, B_STAGE, wfull + 8 * s);
+                        if (++s == PIPE_B_STAGES) { s = 0; ph ^= 1; }
+                    }
+            }
+        } else {                                                        // warps 1..3: the halo of every tile
+            const uint32_t *in = reinterpret_cast<const uint32_t *>(a.in);
+            const int ft = tid - 32;
+            int b = 0;
+            uint32_t ph = 0;
+            for (int64_t tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+                int64_t g_lo;
+                int n;
+                halo_span(a, tile, g_lo, n);
+                mbar_wait(hempty + 8 * b, ph ^ 1);                      // both consumers read their last tap from it
+                const uint32_t hi = halo0 + (uint32_t)b * halo_bytes, lo = hi + plane;
+                // units (pixel, 16-byte chunk q of 8 channels), two per thread in flight
+                const int nu = n * a.W * 8;
+#pragma unroll 1
+                for (int u0 = ft; u0 < nu; u0 += 2 * PIPE_FILL_THREADS) {
+                    uint4 raw[2][4][2];
+#pragma unroll
+                    for (int v = 0; v < 2; ++v) {
+                        const int u = u0 + v * PIPE_FILL_THREADS;
+                        if (u < nu) {
+                            const int64_t gp = g_lo * a.W + (u >> 3);   // pixel of the tall pooled image
+                            const int64_t gr = gp / a.W, img = gr / a.H;
+                            const int iw = (int)(gp - gr * a.W), ih = (int)(gr - img * a.H);
+                            const int64_t p00 = ((img * a.pool_h + 2 * ih) * a.pool_w + 2 * iw) * a.C + (u & 7) * 8;
+                            const int64_t offs[4] = {p00, p00 + a.C, p00 + (int64_t)a.pool_w * a.C, p00 + (int64_t)a.pool_w * a.C + a.C};
+                            pool_load<8>(in, offs, raw[v]);
+                        }
+                    }
+#pragma unroll
+                    for (int v = 0; v < 2; ++v) {
+                        const int u = u0 + v * PIPE_FILL_THREADS;
+                        if (u < nu) {
+                            uint32_t w[8], hw[4], lw[4];
+                            pool_select<8>(raw[v], w);
+                            words_to_planes(w, hw, lw);
+                            const int px = u >> 3, q = u & 7;
+                            const uint32_t o = (uint32_t)px * 128u + ((uint32_t)(q ^ (px & 7)) << 4);
+                            sts128(hi + o, hw[0], hw[1], hw[2], hw[3]);
+                            sts128(lo + o, lw[0], lw[1], lw[2], lw[3]);
+                        }
+                    }
+                }
+                mbar_arrive(hfull + 8 * b);
+                if (++b == PIPE_HALOS) { b = 0; ph ^= 1; }
+            }
+        }
+        return;
+    }
+
+    // ============================ consumers ============================
+    setmaxnreg_inc<PIPE_CONSUMER_REGS>();
+    const int c = wg - 1, t = tid & 127, w = t >> 5, l = t & 31;
+    const int r = 16 * w + (l & 7) + 8 * ((l >> 3) & 1);               // this lane's ldmatrix row of the warpgroup's 64
+    const int half = l >> 4;                                            // and its 16-byte half of each k16 step
+    const int n0 = blockIdx.y * BN;
+    int s = 0, b = 0;
+    uint32_t wph = 0, hph = 0;
+    for (int64_t tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+        int64_t g_lo;
+        int n;
+        halo_span(a, tile, g_lo, n);
+        const int64_t m0 = tile * TBM + 64 * c, m = m0 + r;
+        const bool okr = m < a.M;
+        const int64_t ohw = (int64_t)a.OH * a.OW;
+        const int64_t img = okr ? m / ohw : 0;
+        const int rem = okr ? (int)(m - img * ohw) : 0;
+        const int oh = rem / a.OW, ow = rem - oh * a.OW;
+        const int ih0 = oh * a.SH - a.PT, iw0 = ow * a.SW - a.PL, hb = (int)(img * a.H - g_lo);
+
+        float dm[BN / 2], dl[BN / 2];
+#pragma unroll
+        for (int q = 0; q < BN / 2; ++q) { dm[q] = 0.f; dl[q] = 0.f; }
+        wgmma_fence_operand(dm);
+        wgmma_fence_operand(dl);
+        mbar_wait(hfull + 8 * b, hph);
+        const uint32_t hi = halo0 + (uint32_t)b * halo_bytes;
+
+        int kh = 0, kw = 0;
+        for (int kb = 0; kb < nkb; ++kb) {
+            const int ih = ih0 + kh, iw = iw0 + kw;
+            const int p = okr && ih >= 0 && ih < a.H && iw >= 0 && iw < a.W ? (hb + ih) * a.W + iw : zp;
+            uint32_t ah[4][4], al[4][4];
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk) {
+                const uint32_t o = hi + (uint32_t)p * 128u + ((uint32_t)((2 * kk + half) ^ (p & 7)) << 4);
+                ldsm_x4(o, ah[kk]);
+                ldsm_x4(o + plane, al[kk]);
+            }
+            if (kb == nkb - 1) {                                        // the last read of this halo buffer
+                __syncwarp();
+                if (l == 0) mbar_arrive(hempty + 8 * b);
+            }
+            mbar_wait(wfull + 8 * s, wph);                              // the weights of this tap landed
+            wgmma_fence();
+            const uint64_t db = make_sw128_desc(ring + (uint32_t)s * B_STAGE), dbl = db + ((BN * 128) >> 4);
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk) {
+                wgmma_f16_rs<BN>(dm, ah[kk], db + 2 * kk);              // Ah.Bh
+                wgmma_f16_rs<BN>(dl, ah[kk], dbl + 2 * kk);             // Ah.Bl
+                wgmma_f16_rs<BN>(dl, al[kk], db + 2 * kk);              // Al.Bh
+            }
+            wgmma_commit();
+            wgmma_wait<0>();                                            // the A registers and the stage are free again
+            if (l == 0) mbar_arrive(wempty + 8 * s);
+            if (++s == PIPE_B_STAGES) { s = 0; wph ^= 1; }
+            if (++kw == a.KW) { kw = 0; ++kh; }
+        }
+        wgmma_fence_operand(dm);
+        wgmma_fence_operand(dl);
+        if (++b == PIPE_HALOS) { b = 0; hph ^= 1; }
+        wg_epilogue<ENG_F16, BN>(a, dm, dl, m0, n0, t, inv_scale);
+    }
+}
+
 // halo_rows > 0 (LD_POOL with C = 64 only): the tile's pooled input rows fit in a halo of that many rows.  The tile then
 // takes the 2x2 maximum of each of them once, stages the words in shared memory and fills every tap from there instead of
-// taking the maximum of four global words per tap and value.
+// taking the maximum of four global words per tap and value.  pipe (LD_POOL only): two such halos fit, and the layer runs
+// on the pipelined path gather_pipe.
 template <int ENG, int BN, int MODE>
-__global__ void __launch_bounds__(THREADS, 1)
-conv_gemm_wg_kernel(const ConvArgs a, const unsigned char *__restrict__ wt, float inv_scale, int halo_rows)
+__global__ void __launch_bounds__(MODE == LD_POOL ? POOL_THREADS : THREADS, 1)
+conv_gemm_wg_kernel(const ConvArgs a, const unsigned char *__restrict__ wt, float inv_scale, int halo_rows, int pipe)
 {
     using Cfg = WgCfg<BN>;
     constexpr int KE = ENG == ENG_F16 ? HBK : TBK;                       // k-elements per block
     constexpr int RAW = ENG == ENG_F16 ? 2 : 1;                          // 16-byte input loads per 16-byte operand chunk
     constexpr bool PREFETCH = MODE == LD_F32 || MODE == LD_PACKED;       // raw input held in registers one k-block ahead
+    if constexpr (MODE == LD_POOL) {
+        static_assert(ENG == ENG_F16, "the pooled fill is an engine-3 fill");
+        if (pipe) { gather_pipe<BN>(a, wt, inv_scale, halo_rows); return; }
+        if (threadIdx.x < 128) { setmaxnreg_dec<POOL_IDLE_REGS>(); return; }
+        setmaxnreg_inc<POOL_WG_REGS>();
+    }
+    // the 256 threads of the fill / wgmma loop (warpgroups 1 and 2 of the pooled instance) and their barrier
+    auto fill_sync = [&]() {
+        if constexpr (MODE == LD_POOL) asm volatile("bar.sync 1, 256;" ::: "memory");
+        else __syncthreads();
+    };
     const bool halo = MODE == LD_POOL && halo_rows > 0;
     const int b_stages = halo ? HALO_B_STAGES : B_STAGES, b_ahead = b_stages - 2;
     extern __shared__ unsigned char smem_dyn[];
@@ -203,7 +467,7 @@ conv_gemm_wg_kernel(const ConvArgs a, const unsigned char *__restrict__ wt, floa
     const uint32_t a_ring_u32 = b_ring_u32 + (uint32_t)b_stages * Cfg::B_STAGE;
     const uint32_t halo_u32 = a_ring_u32 + A_STAGES * 2 * A_WG;
 
-    const int tid = threadIdx.x, wg = tid >> 7, t = tid & 127;
+    const int tid = threadIdx.x - (MODE == LD_POOL ? 128 : 0), wg = tid >> 7, t = tid & 127;
     const int64_t m0 = (int64_t)blockIdx.x * TBM + wg * 64;
     const int n0 = blockIdx.y * BN;
     const int nkb = a.K / KE;
@@ -245,12 +509,7 @@ conv_gemm_wg_kernel(const ConvArgs a, const unsigned char *__restrict__ wt, floa
     int64_t g_lo = 0;
     int halo_n = 0, row_hb[4];
     if (halo) {
-        const int64_t ohw = (int64_t)a.OH * a.OW;
-        const int64_t mf = (int64_t)blockIdx.x * TBM, ml = (mf + TBM < a.M ? mf + TBM : a.M) - 1;
-        const int64_t img0 = mf / ohw, img1 = ml / ohw;
-        const int oh0 = (int)(mf - img0 * ohw) / a.OW, oh1 = (int)(ml - img1 * ohw) / a.OW;
-        g_lo = img0 * a.H + max(oh0 * a.SH - a.PT, 0);
-        halo_n = (int)(img1 * a.H + min(oh1 * a.SH - a.PT + a.KH - 1, a.H - 1) - g_lo + 1);
+        halo_span(a, blockIdx.x, g_lo, halo_n);
 #pragma unroll
         for (int i = 0; i < 4; ++i) row_hb[i] = (int)((int64_t)row_img[i] * a.H - g_lo);
     }
@@ -269,7 +528,7 @@ conv_gemm_wg_kernel(const ConvArgs a, const unsigned char *__restrict__ wt, floa
                 pool_max_words(reinterpret_cast<const uint32_t *>(a.in), offs, w);
                 sts128(halo_u32 + (uint32_t)u * 16u, w[0], w[1], w[2], w[3]);
             }
-            __syncthreads();
+            fill_sync();
         }
     }
     // tap of the next k-block to fill: k = (rr * KW + ss) * C + c0
@@ -361,8 +620,8 @@ conv_gemm_wg_kernel(const ConvArgs a, const unsigned char *__restrict__ wt, floa
         if (halo) cp_async_wait<0>();                        // weights of kb landed
         else cp_async_wait<1>();                             // (kb + 1 may still be in flight)
         fence_proxy_async();
-        __syncthreads();
-        issue_b(kb + b_ahead);                               // its stage was read by kb - 2, retired in every warpgroup
+        fill_sync();
+        issue_b(kb + b_ahead);                              // its stage was read by kb - 2, retired in every warpgroup
         wgmma_fence();
         const uint64_t da = make_sw128_desc(a_ring_u32 + (uint32_t)(s * 2 + wg) * A_WG);
         const uint64_t dal = da + ((A_WG / 2) >> 4);
@@ -386,20 +645,7 @@ conv_gemm_wg_kernel(const ConvArgs a, const unsigned char *__restrict__ wt, floa
     wgmma_wait<0>();
     cp_async_wait<0>();
 
-    // ============================ epilogue (from the accumulator registers) ============================
-    const int w = t >> 5, l = t & 31;
-    const int64_t mr = m0 + 16 * w + (l >> 2);
-#pragma unroll
-    for (int i = 0; i < BN / 8; ++i) {
-        const int nb = n0 + 8 * i + 2 * (l & 3);
-        const EpiCoef c = epi_coef(a, nb);
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            const int64_t m = mr + 8 * h;
-            if (m >= a.M) continue;
-            epi_store<ENG>(a, c, m, nb, dm[4 * i + 2 * h] + dl[4 * i + 2 * h], dm[4 * i + 2 * h + 1] + dl[4 * i + 2 * h + 1], inv_scale);
-        }
-    }
+    wg_epilogue<ENG, BN>(a, dm, dl, m0, n0, t, inv_scale);
 }
 
 template <int ENG, int BN, int MODE>
@@ -407,13 +653,21 @@ int launch_wg(const ConvArgs &a, const void *wt, float inv_scale, cudaStream_t s
 {
     using Cfg = WgCfg<BN>;
     auto kern = conv_gemm_wg_kernel<ENG, BN, MODE>;
-    const int halo_rows = MODE == LD_POOL ? iss_gather_halo_rows(a) : 0;
-    const int smem = halo_rows > 0 ? halo_smem(BN, halo_rows, a.W) : Cfg::SMEM;
+    const int pipe_rows = MODE == LD_POOL ? iss_gather_pipe_rows(a) : 0;
+    const int halo_rows = pipe_rows > 0 ? pipe_rows : MODE == LD_POOL ? iss_gather_halo_rows(a) : 0;
+    const int smem = pipe_rows > 0 ? pipe_smem(BN, pipe_rows, a.W) : halo_rows > 0 ? halo_smem(BN, halo_rows, a.W) : Cfg::SMEM;
     ISS_CUDA_OK(iss_optin_smem(reinterpret_cast<const void *>(kern), smem));
     const int64_t gm = (a.M + TBM - 1) / TBM;
     ISS_REQUIRE(gm < (1ll << 31), ISS_ERR_INVALID, "conv_tc: M too large");
     dim3 grid((unsigned)gm, (unsigned)(a.N / BN));
-    kern<<<grid, THREADS, smem, st>>>(a, reinterpret_cast<const unsigned char *>(wt), inv_scale, halo_rows);
+    if (pipe_rows > 0) {                                     // persistent: at most one CTA per SM and n-tile
+        int dev = 0, sms = 0;
+        ISS_CUDA_OK(cudaGetDevice(&dev));
+        ISS_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+        grid.x = (unsigned)(gm < sms ? gm : sms);
+    }
+    const int threads = MODE == LD_POOL ? POOL_THREADS : THREADS;
+    kern<<<grid, threads, smem, st>>>(a, reinterpret_cast<const unsigned char *>(wt), inv_scale, halo_rows, pipe_rows > 0);
     ISS_CUDA_OK(cudaGetLastError());
     iss_count_launch();
     return ISS_OK;
@@ -736,6 +990,20 @@ extern "C" int iss_gather_halo_smem(int H, int W, int OH, int OW, int KH, int KW
 int iss_gather_halo_rows(const ConvArgs &a)
 {
     return iss_gather_halo_smem(a.H, a.W, a.OH, a.OW, a.KH, a.KW, a.SH, a.PT, a.C, a.N) ? iss_gather_halo_rows_bound(a.H, a.OH, a.OW, a.KH, a.SH, a.PT) : 0;
+}
+
+// Shared memory of a pooled gather-kernel layer (LD_POOL) on the pipelined path, 0 where it keeps another path: the layer
+// takes the halo (64 input channels, more than one tap) and two halo buffers fit next to the three-stage weight ring.
+extern "C" int iss_gather_pipe_smem(int H, int W, int OH, int OW, int KH, int KW, int SH, int PT, int C, int N)
+{
+    if (C != HBK || KH * KW == 1) return 0;
+    const int smem = pipe_smem(f16_bn_for(N), iss_gather_halo_rows_bound(H, OH, OW, KH, SH, PT), W);
+    return smem <= MAX_SMEM ? smem : 0;
+}
+
+int iss_gather_pipe_rows(const ConvArgs &a)
+{
+    return iss_gather_pipe_smem(a.H, a.W, a.OH, a.OW, a.KH, a.KW, a.SH, a.PT, a.C, a.N) ? iss_gather_halo_rows_bound(a.H, a.OH, a.OW, a.KH, a.SH, a.PT) : 0;
 }
 
 // Does the slab kernel take this engine-3 layer?  Un-padded, stride-1 'valid' convolution, 64 -> 64 channels, no

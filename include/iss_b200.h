@@ -354,6 +354,11 @@ int iss_gather_halo_rows_bound(int H, int OH, int OW, int KH, int SH, int PT);
  * input width W and a KH x KW filter; 0 when the layer keeps the global-memory
  * operand fill (C != 64, one tap, or the halo does not fit in shared memory). */
 int iss_gather_halo_smem(int H, int W, int OH, int OW, int KH, int KW, int SH, int PT, int C, int N);
+/* Shared memory (bytes) of the pipelined form of that layer: two such halos,
+ * restaged as hi / lo planes, next to a three-stage weight ring, so that the
+ * halo of the next tile is staged while the tensor cores work on this one; 0
+ * when the layer keeps the single halo or the global-memory fill. */
+int iss_gather_pipe_smem(int H, int W, int OH, int OW, int KH, int KW, int SH, int PT, int C, int N);
 
 #ifdef __cplusplus
 }
