@@ -67,6 +67,10 @@ extern "C" int iss_mlp_forward(iss_ctx *ctx, iss_mlp *m, const float *d_x, int64
     ISS_REQUIRE(ctx && m, ISS_ERR_INVALID, "iss_mlp_forward: NULL handle");
     if (n_rows <= 0) return ISS_OK;
     ISS_REQUIRE(d_x && d_y && d_work && work_bytes >= iss_mlp_workspace_bytes(m, n_rows), ISS_ERR_INVALID, "iss_mlp_forward: bad buffer");
+    // the fp32 kernels read rows with float4 loads (conv_gemm_f32_kernel when C % 8 == 0, dense_small_n_kernel when
+    // K % 4 == 0) and store them with float4 stores, without checking the base pointers
+    ISS_REQUIRE(((uintptr_t)d_x | (uintptr_t)d_y | (uintptr_t)d_work) % 16 == 0, ISS_ERR_INVALID,
+                "iss_mlp_forward: d_x, d_y and d_work must be 16-byte aligned");
     ISS_CUDA_OK(cudaSetDevice(ctx->device));
     cudaStream_t st = iss_stream(stream);
     const size_t half = (size_t)((n_rows * m->max_dim * 4 + 255) / 256 * 256);

@@ -146,6 +146,8 @@ class MlpModel:
         """x: [n, in_dim] numpy or CUDA tensor -> numpy float32 [n, out_dim] (keras predict contract)."""
         t = x if isinstance(x, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(x, dtype=np.float32))
         t = t.to(self.ctx.device).contiguous()
+        if t.data_ptr() % 16:                       # a view at an odd offset: iss_mlp_forward needs 16-byte rows
+            t = t.clone()
         n = t.shape[0]
         y = torch.empty((n, self.out_dim), dtype=torch.float32, device=self.ctx.device)
         if n:

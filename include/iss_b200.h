@@ -330,7 +330,8 @@ int iss_mlp_create(iss_ctx *ctx, const iss_layer_desc *layers, int n_layers, con
 int iss_mlp_destroy(iss_mlp *mlp);
 int iss_mlp_out_dim(const iss_mlp *mlp);
 int64_t iss_mlp_workspace_bytes(const iss_mlp *mlp, int64_t n_rows);
-/* d_x: float32 [n_rows][in_dim]; d_y: float32 [n_rows][out_dim]. */
+/* d_x: float32 [n_rows][in_dim]; d_y: float32 [n_rows][out_dim].  d_x, d_y and d_work must be
+ * 16-byte aligned (ISS_ERR_INVALID otherwise). */
 int iss_mlp_forward(iss_ctx *ctx, iss_mlp *mlp, const float *d_x, int64_t n_rows, float *d_y,
                     void *d_work, int64_t work_bytes, void *stream);
 

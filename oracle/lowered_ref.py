@@ -7,7 +7,7 @@ the blob -- so the folded BatchNorm is the one the kernels use:
   Conv2D     explicit pads / strides, then the epilogue bias -> pre-affine -> ReLU -> sigmoid -> post-affine
   Dense      the same epilogue on [n, cin] (the NHWC flatten order)
   MaxPool    -inf padding
-  softmax    on the head only, then the non-finite override (rows of non-finite patches = 0.5)
+  softmax    on the head only, then the non-finite override (rows of non-finite patches = 0.5, E = 0)
 
 The patch z-normalisation is the one ``patch_stats_kernel`` computes: float64 sums in its lane order, mean and
 population std rounded to float32; the network input is (x - mu) / sigma of those float32 values, taken exactly.
@@ -23,6 +23,17 @@ for layers on the fp32 CUDA cores and 2^-22 for the first layer (its input is ro
 subnormal range adds an absolute term: fp16 lo parts are subnormal below 2^-14, so a split value carries up to 2^-25
 absolute error there.  The bound is a scale, not a proof: tests compare |got - ref| <= c . E with a constant c
 calibrated on the unmodified kernels.
+
+The head's softmax (softmax_head_kernel: max subtraction, expf, an fp32 sum over k = 0 .. K-1, one division) carries
+the logits' bound to first order, p_k (E_k + sum_j p_j E_j), and adds its own rounding, relative to p_k: the rounded
+z_k = l_k - max (U32 |z_k|, and the p-weighted mean of those in the sum), two expf of at most 2 ulp each (U_EXP), K - 1
+fp32 additions and the division (U32 each), plus one subnormal ulp where an exponential underflows.
+
+The MLP of VoiceFemininityScoring is the same Dense stack on the fp32 kernels: ``eval_layers(..., mode=0,
+first=False)`` evaluates its lowered descs with u = U32 on every layer.
+
+``kernel_names`` mirrors the dispatch (iss_conv_kernel, iss_prepare_weights, iss_slab_covers and plan_forward): the
+CUDA kernels one forward of a lowered network launches in a GEMM mode.
 """
 from fractions import Fraction
 
@@ -40,6 +51,8 @@ U_SPLIT = 2.0 ** -22       # engines 2 and 3: hi / lo split of both operands (th
 U32 = 2.0 ** -24           # fp32 CUDA cores
 U_FIRST = 2.0 ** -22       # first layer: z rounded to fp32 before the products, taps accumulated in fp32 (a few U32)
 ABS_SPLIT = 2.0 ** -25     # absolute error of an fp16 hi + lo pair whose lo part is subnormal
+U_EXP = 2.0 ** -22         # expf without fast-math: at most 2 ulp
+ABS_EXP = 2.0 ** -149      # one subnormal ulp: an exponential (or a probability) that underflows
 
 
 # ------------------------------------------------------------------ patches (patch_index_kernel + patch_stats_kernel)
@@ -99,9 +112,10 @@ def patch_inputs(mspec, nmel, ranges, edge_left=True, edge_right=True):
 
 
 # ------------------------------------------------------------------ layers
-def _engine_u(d, li, in_shape, mode):
-    """Unit error of the engine a layer runs on (the dispatch of cnn.cu / conv_gemm.cu, by shape)."""
-    if li == 0:
+def _engine_u(d, li, in_shape, mode, first=True):
+    """Unit error of the engine a layer runs on (the dispatch of cnn.cu / conv_gemm.cu, by shape).  first: layer 0
+    is the CNN's first layer, which reads the z-normalised patch."""
+    if li == 0 and first:
         return U_FIRST
     if d['kind'] == LAYER_MAXPOOL or mode == 0 or d['flags'] & F_SIGMOID:
         return U32                                     # only the fp32 kernels evaluate a sigmoid
@@ -161,10 +175,25 @@ def _maxpool(x, d):
     return y.permute(0, 2, 3, 1).contiguous().numpy()
 
 
-def eval_layers(lowered, x, E=None, mode=3, start=0, stop=None):
+def softmax(logits, E=None):
+    """Softmax over the last axis of float64 logits [n, K] with the bound of softmax_head_kernel: the logits' bound E
+    (zeros when None) carried to first order plus the kernel's own rounding (module docstring).  Returns (p, E_p)."""
+    lg = np.asarray(logits, dtype=np.float64)
+    E = np.zeros_like(lg) if E is None else np.asarray(E, dtype=np.float64)
+    z = lg - lg.max(axis=-1, keepdims=True)
+    e = np.exp(z)
+    p = e / e.sum(axis=-1, keepdims=True)
+    K = lg.shape[-1]
+    az = np.abs(z)
+    rel = U32 * az + U32 * (p * az).sum(axis=-1, keepdims=True) + 2 * U_EXP + K * U32
+    return p, p * (E + (p * E).sum(axis=-1, keepdims=True)) + p * rel + 2 * ABS_EXP
+
+
+def eval_layers(lowered, x, E=None, mode=3, start=0, stop=None, first=True):
     """Layers [start, stop) of a LoweredModel on x (float64: [n, H, W, C], or [n, K] after a Dense) with bound E
-    (zeros when None).  mode: the GEMM engine (0 = fp32 CUDA cores, 2 / 3 = the split engines).  Returns (y, E) as
-    float64 numpy arrays, NHWC or [n, K]; the head's softmax, if any, is applied to y (E is left as the logits')."""
+    (zeros when None).  mode: the GEMM engine (0 = fp32 CUDA cores, 2 / 3 = the split engines).  first: layer 0 is the
+    CNN's first layer (False for an MLP, whose layers all run on the fp32 kernels).  Returns (y, E) as float64 numpy
+    arrays, NHWC or [n, K]; the head's softmax, if any, is applied to y and E."""
     descs, blob = lowered.descs, np.asarray(lowered.blob, dtype=np.float32)
     stop = len(descs) if stop is None else stop
     x = np.asarray(x, dtype=np.float64)
@@ -174,7 +203,7 @@ def eval_layers(lowered, x, E=None, mode=3, start=0, stop=None):
         if d['kind'] == LAYER_MAXPOOL:
             x, E = _maxpool(x, d), _maxpool(E, d)      # max |a_i - b_i| bounds |max a - max b|
             continue
-        u = _engine_u(d, li, x.shape, mode)
+        u = _engine_u(d, li, x.shape, mode, first)
         K = d['cin'] if d['kind'] == LAYER_DENSE else d['kh'] * d['kw'] * d['cin']
         w = blob[d['w_off']:d['w_off'] + K * d['cout']].astype(np.float64)
         slack = E + u * np.abs(x) + (ABS_SPLIT if u == U_SPLIT else 0.0)
@@ -187,8 +216,7 @@ def eval_layers(lowered, x, E=None, mode=3, start=0, stop=None):
             y, E = _conv(x, w, d), _conv(slack, np.abs(w), d)
         x, E = _epilogue(d, blob, y, E)
         if d['flags'] & F_SOFTMAX:
-            z = x - x.max(axis=1, keepdims=True)
-            x = np.exp(z) / np.exp(z).sum(axis=1, keepdims=True)
+            x, E = softmax(x, E)
     return x, E
 
 
@@ -200,3 +228,130 @@ def evaluate(lowered, mspec, ranges, mode=3, edge_left=True, edge_right=True):
     y, E = y.reshape(len(y), -1), E.reshape(len(E), -1)
     y[~finite], E[~finite] = 0.5, 0.0
     return y, E
+
+
+# ------------------------------------------------------------------ dispatch mirror (conv_gemm.cu, conv_gemm_tc.cu, cnn.cu)
+K_F32, K_F32_FIRST, K_FIRST_DIRECT, K_SMALL_N, K_TF32, K_F16, K_SLAB = \
+    'f32', 'f32_first', 'first_direct', 'small_n', 'tf32', 'f16', 'slab'
+_SLAB_ROWS_MAX = (227 * 1024 - 1024 - 4 * 2 * 64 * 128) // 256      # one slab next to a four-stage weight ring
+
+
+def _layer_args(lowered):
+    """Per layer, the ConvArgs fields the dispatch reads (plan_forward's first loop), with the layer's shapes."""
+    h, w, c = lowered.in_h, lowered.in_w, 1
+    out = []
+    for li, d in enumerate(lowered.descs):
+        H, W, C = h, w, c
+        if d['kind'] == LAYER_DENSE:
+            h, w, c = 1, 1, d['cout']
+            a = dict(K=d['cin'], C=d['cin'], H=1, W=1, OH=1, OW=1, KH=1, KW=1, SH=1, SW=1, PT=0, PL=0)
+        else:
+            h = (H + d['pad_top'] + d['pad_bottom'] - d['kh']) // d['sh'] + 1
+            w = (W + d['pad_left'] + d['pad_right'] - d['kw']) // d['sw'] + 1
+            c = d['cout'] if d['kind'] == LAYER_CONV2D else C
+            a = dict(K=d['kh'] * d['kw'] * C, C=C, H=H, W=W, OH=h, OW=w, KH=d['kh'], KW=d['kw'], SH=d['sh'], SW=d['sw'],
+                     PT=d['pad_top'], PL=d['pad_left'])
+        # iss_prepare_weights: engine 2's image for C, K, N multiples of 32, engine 3's also with C, N multiples of 64
+        tiled = li > 0 and d['kind'] != LAYER_MAXPOOL and a['C'] % 32 == 0 and a['K'] % 32 == 0 and d['cout'] % 32 == 0
+        a.update(d=d, li=li, N=c, flags=d['flags'] & ~F_SOFTMAX, tiled=tiled,
+                 f16=tiled and a['C'] % 64 == 0 and c % 64 == 0, in_packed=False, out_packed=False, pool_h=0, pool_w=0,
+                 first=False)
+        out.append(a)
+    return out
+
+
+def conv_kernel(a, mode):
+    """iss_conv_kernel (conv_gemm.cu) for the fields of ``_layer_args``."""
+    if a['li'] == 0:
+        return K_FIRST_DIRECT if a['C'] == 1 and a['N'] in (16, 32, 64, 128) else K_F32_FIRST
+    if (a['KH'] == 1 and a['KW'] == 1 and a['SH'] == 1 and a['SW'] == 1 and a['PT'] == 0 and a['PL'] == 0 and
+            a['N'] <= 8 and a['K'] % 4 == 0 and a['K'] == a['C'] and a['K'] * a['N'] * 4 <= 48 * 1024 and
+            not a['in_packed'] and not a['out_packed']):
+        return K_SMALL_N
+    if mode == 0 or not a['tiled'] or a['flags'] & F_SIGMOID:
+        return K_F32
+    if mode == 3 and a['f16']:
+        slab = (a['C'] == 64 and a['N'] == 64 and a['K'] == a['KH'] * a['KW'] * a['C'] and a['pool_h'] == 0 and
+                a['SH'] == 1 and a['SW'] == 1 and a['PT'] == 0 and a['PL'] == 0 and a['OH'] == a['H'] - a['KH'] + 1 and
+                a['OW'] == a['W'] - a['KW'] + 1 and (256 + (a['KH'] - 1) * a['W'] + a['KW'] - 1 + 7) // 8 * 8 <= _SLAB_ROWS_MAX)
+        pool_ok = a['pool_h'] == 0 or (not a['first'] and a['in_packed'] and a['pool_h'] // 2 == a['H'] and
+                                       a['pool_w'] // 2 == a['W'])
+        if pool_ok and (not a['first'] or slab):
+            return K_SLAB if slab else K_F16
+    return K_TF32
+
+
+def _is_f16(k):
+    return k in (K_F16, K_SLAB)
+
+
+def _kernel_name(a, k):
+    N = a['N']
+    if k == K_FIRST_DIRECT:
+        return 'conv_first_direct_kernel'
+    if k in (K_F32, K_F32_FIRST):
+        return 'conv_gemm_f32_kernel<%d,%s>' % (64 if N <= 64 else 128, 'true' if k == K_F32_FIRST else 'false')
+    if k == K_SMALL_N:
+        return 'dense_small_n_kernel'
+    if k == K_SLAB:
+        return 'conv_slab_kernel<%d>' % (3 if a['first'] else int(a['in_packed']))
+    if k == K_F16:
+        return 'conv_gemm_wg_kernel<1,%d,%d>' % (128 if N % 128 == 0 else 64, 2 if a['pool_h'] else int(a['in_packed']))
+    return 'conv_gemm_wg_kernel<0,%d,0>' % (128 if N % 128 == 0 else 64 if N % 64 == 0 else 32)
+
+
+def plan(lowered, mode, fuse_first=True, fuse_pool=True):
+    """plan_forward (cnn.cu): per layer (kernel name, or None for a pooling folded into the next convolution or a
+    first layer folded into the second), for a batch whose patches span few enough frames for the fused first layer's
+    map (contiguous ascending ranges of up to 8192 patches).  fuse_first / fuse_pool: ISS_B200_FUSE_FIRST /
+    ISS_B200_FUSE_POOL not '0'."""
+    args = _layer_args(lowered)
+    n = len(args)
+
+    def reads_packed(j):
+        return _is_f16(conv_kernel(dict(args[j], in_packed=True), mode))
+
+    names = [None] * n
+    packed, pool_h, pool_w, first_fused = False, 0, 0, False
+    for li, a in enumerate(args):
+        d = a['d']
+        if d['kind'] == LAYER_MAXPOOL:
+            nx = args[li + 1]['d'] if li + 1 < n else None
+            if (packed and fuse_pool and nx is not None and (d['kh'], d['kw'], d['sh'], d['sw']) == (2, 2, 2, 2) and
+                    d['pad_top'] == d['pad_left'] == d['pad_bottom'] == d['pad_right'] == 0 and
+                    nx['kind'] == LAYER_CONV2D and nx['pad_bottom'] == 0 and nx['pad_right'] == 0 and
+                    _is_f16(conv_kernel(dict(args[li + 1], in_packed=True, pool_h=a['H'], pool_w=a['W']), mode))):
+                pool_h, pool_w = a['H'], a['W']
+                continue
+            names[li] = 'maxpool_nhwc_kernel<%s>' % ('uint4' if packed else 'float4' if a['C'] % 4 == 0 else 'float')
+            continue
+        a.update(in_packed=packed, pool_h=pool_h, pool_w=pool_w)
+        pool_h = pool_w = 0
+        j = li + 1
+        while j < n and args[j]['d']['kind'] == LAYER_MAXPOOL:
+            j += 1
+        pools_vec4 = all(args[p]['C'] % 4 == 0 for p in range(li + 1, j))
+        a['out_packed'] = j < n and pools_vec4 and reads_packed(j) and \
+            (_is_f16(conv_kernel(a, mode)) or conv_kernel(a, mode) == K_FIRST_DIRECT)
+        if li == 0:
+            d1 = args[1]['d'] if n > 1 else None
+            first_fused = (a['out_packed'] and fuse_first and d['sh'] == 1 and d['sw'] == 1 and
+                           d['pad_top'] == d['pad_left'] == d['pad_bottom'] == d['pad_right'] == 0 and
+                           not d['flags'] & F_SIGMOID and d1['kind'] == LAYER_CONV2D and d1['pad_bottom'] == 0 and
+                           d1['pad_right'] == 0 and _is_f16(conv_kernel(dict(args[1], in_packed=True, first=True), mode)))
+            if first_fused:
+                continue
+        if li == 1 and first_fused:
+            a['first'] = True
+        names[li] = _kernel_name(a, conv_kernel(a, mode))
+        packed = a['out_packed']
+    return names
+
+
+def kernel_names(lowered, mode, fuse_first=True, fuse_pool=True):
+    """Names (as the profiler shows them, white space removed) of the CUDA kernels one CnnModel.forward launches."""
+    names = {'patch_index_kernel', 'patch_stats_kernel', 'softmax_head_kernel'}
+    p = plan(lowered, mode, fuse_first, fuse_pool)
+    if p[0] is None:
+        names |= {'first_linear_kernel', 'first_coef_kernel'}
+    return names | {k for k in p if k is not None}

@@ -284,3 +284,48 @@ def make_mspec(kind, L=1600, seed=0):
         m[400:560] = np.float32(-7.25)
         m[900:1000] = np.float32(0)
     return m
+
+
+# ------------------------------------------------------------------ MLPs (the Dense stack of VoiceFemininityScoring)
+def mlp_config(in_dim, layers, seed=0):
+    """Keras-style Sequential (config, weights) of Dense layers; each entry of ``layers``: dict(units, bias=True,
+    bn='none' | 'pre' (BatchNorm before the activation) | 'post' (after it), act='linear' | 'relu' | 'sigmoid')."""
+    rng = np.random.default_rng(seed)
+    L = [{'class_name': 'InputLayer', 'config': {'name': 'in', 'batch_input_shape': [None, in_dim]}}]
+    W, cin = {}, in_dim
+    for i, spec in enumerate(layers):
+        units, bias, bn, act = spec['units'], spec.get('bias', True), spec.get('bn', 'none'), spec.get('act', 'linear')
+        name = 'dense_%d' % i
+        W[name + '/kernel'] = (rng.standard_normal((cin, units)) * np.sqrt(2.0 / cin)).astype(np.float32)
+        if bias:
+            W[name + '/bias'] = rng.normal(0, 0.1, units).astype(np.float32)
+        L.append({'class_name': 'Dense', 'config': {'name': name, 'units': units, 'use_bias': bias,
+                                                    'activation': 'linear' if bn == 'pre' else act}})
+        if bn != 'none':
+            b = 'bn_%d' % i
+            W[b + '/gamma'] = rng.uniform(0.8, 1.2, units).astype(np.float32)
+            W[b + '/beta'] = rng.normal(0, 0.1, units).astype(np.float32)
+            W[b + '/moving_mean'] = rng.normal(0, 0.2, units).astype(np.float32)
+            W[b + '/moving_variance'] = rng.uniform(0.5, 1.5, units).astype(np.float32)
+            L.append({'class_name': 'BatchNormalization', 'config': {'name': b, 'axis': -1, 'epsilon': 1e-3}})
+            if bn == 'pre' and act != 'linear':
+                L.append({'class_name': 'Activation', 'config': {'name': 'act_%d' % i, 'activation': act}})
+        cin = units
+    return {'class_name': 'Sequential', 'config': {'name': 'mlp', 'layers': L}}, W
+
+
+# 1 to 4 Dense layers over widths 256, 100, 37 and 1: bias and none, BatchNorm before and after the activation, linear /
+# relu / sigmoid.  Which fp32 kernel a layer takes (conv_gemm.cu): dense_small_n_kernel for N <= 8 and K % 4 == 0, else
+# conv_gemm_f32_kernel, with scalar A loads for K % 8 != 0 and scalar B loads / stores for N % 4 != 0.
+MLP_CASES = {
+    'd1_256_1_sigmoid': (256, [dict(units=1, act='sigmoid')]),
+    'd2_256_100_1': (256, [dict(units=100, act='relu', bn='post'), dict(units=1, act='sigmoid')]),
+    'd3_256_37_100_1': (256, [dict(units=37, bias=False, bn='pre', act='relu'), dict(units=100, act='relu', bn='post'),
+                              dict(units=1, bias=False)]),
+    'd4_256_100_37_8_1': (256, [dict(units=100, bn='pre', act='relu'), dict(units=37, act='sigmoid'),
+                                dict(units=8, act='relu', bn='post'), dict(units=1, act='sigmoid')]),
+    'd2_37_100_3': (37, [dict(units=100, act='relu'), dict(units=3, bias=False, bn='pre', act='sigmoid')]),
+    'd2_100_37_1': (100, [dict(units=37, act='relu', bn='pre'), dict(units=1)]),
+    'd3_256_256_128_1': (256, [dict(units=256, act='relu', bn='post'), dict(units=128, act='relu'),
+                               dict(units=1, act='sigmoid')]),
+}

@@ -20,6 +20,7 @@ split-half words decode to exactly hi + lo of its fp32 output; the fp16 range of
 import json
 import os
 import re
+import time
 
 import numpy as np
 import pytest
@@ -57,6 +58,25 @@ def _norm(name):
     return re.sub(r'\s|\(int\)|\(bool\)|\(anonymousnamespace\)::', '', name)
 
 
+def traced(run):
+    """(run(), the names of the CUDA kernels it launched) from a torch.profiler trace; the names are None when the trace
+    holds no kernels.  run() executes twice: in the profiler's warm-up step, whose records are discarded, and then,
+    after a pause, recorded.  A trace that begins with the launches can lose the first kernels of a short run (a probe
+    forward was seen three times running without its first three kernels), so the recorded run starts only once the
+    activity tracing has been running for a while."""
+    from torch.profiler import ProfilerActivity, profile, schedule
+    with profile(activities=[ProfilerActivity.CUDA], schedule=schedule(wait=0, warmup=1, active=1, repeat=1)) as prof:
+        run()
+        torch.cuda.synchronize()
+        prof.step()
+        time.sleep(0.02)
+        out = run()
+        torch.cuda.synchronize()
+        prof.step()
+    names = sorted({_norm(e.name) for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA})
+    return out, names or None
+
+
 def _forward(rt, low, dm, ranges, mode, fuse, profile=False):
     """Output of the operator ([n, 8] numpy) and, with profile, the names of the CUDA kernels it launched (None when
     the profiler records no kernels)."""
@@ -68,12 +88,7 @@ def _forward(rt, low, dm, ranges, mode, fuse, profile=False):
         net = rt['engine'].CnnModel(rt['ctx'], low)
         names = None
         if profile:
-            from torch.profiler import ProfilerActivity, profile as prof_ctx
-            with prof_ctx(activities=[ProfilerActivity.CUDA]) as prof:
-                out = net.forward(dm, ranges)
-                torch.cuda.synchronize()
-            names = sorted({_norm(e.name) for e in prof.events()
-                            if e.device_type == torch.autograd.DeviceType.CUDA}) or None
+            out, names = traced(lambda: net.forward(dm, ranges))
         else:
             out = net.forward(dm, ranges)
         out = out.cpu().numpy().astype(np.float64)

@@ -86,11 +86,8 @@ class Net:
                                              L.ptr(emb), L.ptr(work), work.numel(), None), 'iss_resnet_embed')
                 torch.cuda.synchronize()
             if profile:
-                from torch.profiler import ProfilerActivity, profile as prof_ctx
-                with prof_ctx(activities=[ProfilerActivity.CUDA]) as prof:
-                    run()
-                names = {m.group(1) for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA
-                         for m in [KERNEL_RE.search(_norm(e.name))] if m}
+                from test_layer_probes_gpu import traced
+                names = {m.group(1) for n in traced(run)[1] or [] for m in [KERNEL_RE.search(_norm(n))] if m}
             else:
                 run()
         finally:
