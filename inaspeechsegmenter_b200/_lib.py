@@ -36,7 +36,7 @@ F_BIAS, F_AFFINE_PRE, F_RELU, F_AFFINE_POST, F_SOFTMAX, F_SIGMOID = 1, 2, 4, 8, 
 PCM_F32, PCM_S16 = 0, 1
 FFT_FP32, FFT_FP64 = 0, 1
 GEMM_FP32, GEMM_TC_TS, GEMM_TC_F16 = 0, 2, 3     # fp32 CUDA cores | 3xTF32 wgmma | fp16-split wgmma (default)
-ABI_VERSION = 5                       # == ISS_ABI_VERSION in include/iss_b200.h
+ABI_VERSION = 6                       # == ISS_ABI_VERSION in include/iss_b200.h
 
 # name -> (restype, argtypes); must list every symbol include/iss_b200.h declares
 _vp, _i, _i64, _d = _c.c_void_p, _c.c_int, _c.c_int64, _c.c_double
@@ -53,11 +53,15 @@ SIGNATURES = {
     'iss_sidekit_features': (_i, [_vp, _vp, _i, _i64, _i, _vp, _vp, _vp, _vp]),
     'iss_sidekit_features_multi': (_i, [_vp, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     'iss_loge_stats': (_i, [_vp, _vp, _i64, _vp, _vp]),
+    'iss_loge_stats_multi': (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp]),
     'iss_set_energy_viterbi_serial': (_i, [_i]),
     'iss_energy_viterbi': (_i, [_vp, _vp, _i64, _vp, _d, _vp, _vp, _d, _i, _vp, _vp, _vp]),
     'iss_energy_viterbi_multi': (_i, [_vp, _vp, _vp, _i, _vp, _d, _vp, _vp, _d, _i, _vp, _vp, _vp, _vp]),
     'iss_viterbi_segments': (_i, [_vp, _vp, _i, _vp, _i, _vp, _d, _vp, _vp, _vp]),
     'iss_viterbi_work_bytes': (_i64, [_i64, _i]),
+    'iss_viterbi_online': (_i, [_vp, _i, _i, _vp, _vp, _i64, _vp, _d, _vp, _vp, _d, _vp, _vp, _i64, _i64, _vp, _i64, _vp,
+                                _vp, _vp]),
+    'iss_viterbi_online_work_bytes': (_i64, [_i]),
     'iss_energy_transfer': (_i, [_vp, _vp, _i64, _vp, _d, _vp, _vp, _vp, _vp, _vp]),
     'iss_energy_forward': (_i, [_vp, _vp, _i64, _vp, _d, _vp, _vp, _d, _vp, _vp, _vp, _vp, _vp]),
     'iss_energy_emit': (_i, [_vp, _i64, _i, _i, _vp, _vp, _vp]),

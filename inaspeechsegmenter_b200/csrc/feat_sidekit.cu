@@ -299,11 +299,9 @@ loge_stats_finalize_kernel(const double *__restrict__ partials, const FeatRec *_
 
 // Same arithmetic as the fused per-tile partials above: warp w of a tile sums the
 // frames w, w+8, ... in order, the tile sums its 8 warps in order.
-__global__ void __launch_bounds__(128)
-loge_tile_partials_kernel(const float *__restrict__ loge, int64_t L, int64_t ntiles, double *__restrict__ partials)
+__device__ __forceinline__ void loge_tile_partial(const float *__restrict__ loge, int64_t L, int64_t tile,
+                                                  double *__restrict__ partials)
 {
-    const int64_t tile = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (tile >= ntiles) return;
     const int64_t f0 = tile * FR;
     const int nfr = (int)min((int64_t)FR, L - f0);
     double s = 0.0, c = 0.0;
@@ -315,8 +313,29 @@ loge_tile_partials_kernel(const float *__restrict__ loge, int64_t L, int64_t nti
         }
         s += sw; c += cw;
     }
-    partials[2 * tile] = s;
-    partials[2 * tile + 1] = c;
+    partials[0] = s;
+    partials[1] = c;
+}
+
+__global__ void __launch_bounds__(128)
+loge_tile_partials_kernel(const float *__restrict__ loge, int64_t L, int64_t ntiles, double *__restrict__ partials)
+{
+    const int64_t tile = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (tile >= ntiles) return;
+    loge_tile_partial(loge, L, tile, partials + 2 * tile);
+}
+
+// The tiles of many sequences (recording r: loge_off / n_frames / tile_off of recs[r]), each tiled from its own start.
+__global__ void __launch_bounds__(128)
+loge_tile_partials_multi_kernel(const float *__restrict__ loge, const FeatRec *__restrict__ recs, int n_rec,
+                                int64_t ntiles, double *__restrict__ partials)
+{
+    const int64_t tile = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (tile >= ntiles) return;
+    int lo = 0, hi = n_rec;                            // recs[lo].tile_off <= tile < recs[hi].tile_off
+    while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (recs[mid].tile_off <= tile) lo = mid; else hi = mid; }
+    const FeatRec r = recs[lo];
+    loge_tile_partial(loge + r.loge_off, r.n_frames, tile - r.tile_off, partials + 2 * tile);
 }
 
 }  // namespace
@@ -330,6 +349,19 @@ static int ensure_partials(iss_ctx *ctx, int64_t ntiles)
         cudaError_t e = cudaMalloc(&ctx->d_partials, (size_t)cap * 2 * sizeof(double));
         if (e != cudaSuccess) { iss_set_error("cudaMalloc partials: %s", cudaGetErrorString(e)); return ISS_ERR_NOMEM; }
         ctx->partials_cap = cap;
+    }
+    return ISS_OK;
+}
+
+static int ensure_recs(iss_ctx *ctx, int n_rec)
+{
+    if (n_rec + 1 > ctx->recs_cap) {
+        if (ctx->d_recs) ISS_CUDA_OK(cudaFree(ctx->d_recs));
+        ctx->d_recs = nullptr; ctx->recs_cap = 0;
+        const int64_t cap = n_rec + 1 + n_rec / 2 + 64;
+        cudaError_t e = cudaMalloc(&ctx->d_recs, (size_t)cap * sizeof(FeatRec));
+        if (e != cudaSuccess) { iss_set_error("cudaMalloc recording table: %s", cudaGetErrorString(e)); return ISS_ERR_NOMEM; }
+        ctx->recs_cap = cap;
     }
     return ISS_OK;
 }
@@ -470,13 +502,9 @@ extern "C" int iss_sidekit_features_multi(iss_ctx *ctx, int n_rec, const void *c
         const int prc = ensure_partials(ctx, ntiles);
         if (prc != ISS_OK) return prc;
     }
-    if (n_rec + 1 > ctx->recs_cap) {
-        if (ctx->d_recs) ISS_CUDA_OK(cudaFree(ctx->d_recs));
-        ctx->d_recs = nullptr; ctx->recs_cap = 0;
-        const int64_t cap = n_rec + 1 + n_rec / 2 + 64;
-        cudaError_t e = cudaMalloc(&ctx->d_recs, (size_t)cap * sizeof(FeatRec));
-        if (e != cudaSuccess) { iss_set_error("cudaMalloc recording table: %s", cudaGetErrorString(e)); return ISS_ERR_NOMEM; }
-        ctx->recs_cap = cap;
+    {
+        const int rrc = ensure_recs(ctx, n_rec);
+        if (rrc != ISS_OK) return rrc;
     }
     const FeatRec *d_recs = reinterpret_cast<const FeatRec *>(ctx->d_recs);
     ISS_CUDA_OK(cudaMemcpyAsync(ctx->d_recs, recs.data(), sizeof(FeatRec) * (n_rec + 1), cudaMemcpyHostToDevice, st));
@@ -505,4 +533,33 @@ extern "C" int iss_sidekit_features(iss_ctx *ctx, const void *d_pcm, int pcm_for
     const int64_t zero = 0;
     return iss_sidekit_features_multi(ctx, 1, &d_pcm, &n_samples, pcm_format, fft_precision, d_mspec, &zero, d_loge, &zero,
                                       d_loge_stats, stream);
+}
+
+extern "C" int iss_loge_stats_multi(iss_ctx *ctx, const float *d_loge, const int64_t *h_loge_off, const int64_t *h_len,
+                                    int n_seq, double *d_loge_stats, void *stream)
+{
+    ISS_REQUIRE(ctx && d_loge_stats && h_loge_off && h_len && n_seq >= 1, ISS_ERR_INVALID, "iss_loge_stats_multi: bad argument");
+    ISS_CUDA_OK(cudaSetDevice(ctx->device));
+    cudaStream_t st = iss_stream(stream);
+    std::vector<FeatRec> recs(n_seq + 1);
+    int64_t ntiles = 0;
+    for (int i = 0; i < n_seq; ++i) {
+        ISS_REQUIRE(h_len[i] >= 1 && h_loge_off[i] >= 0, ISS_ERR_INVALID, "iss_loge_stats_multi: sequence %d is empty", i);
+        recs[i] = FeatRec{nullptr, h_len[i], 0, h_loge_off[i], ntiles, 0};
+        ntiles += (h_len[i] + FR - 1) / FR;
+    }
+    recs[n_seq] = FeatRec{nullptr, 0, 0, 0, ntiles, 0};
+    ISS_REQUIRE(d_loge, ISS_ERR_INVALID, "iss_loge_stats_multi: NULL buffer");
+    int rc = ensure_partials(ctx, ntiles);
+    if (rc != ISS_OK) return rc;
+    rc = ensure_recs(ctx, n_seq);
+    if (rc != ISS_OK) return rc;
+    FeatRec *d_recs = reinterpret_cast<FeatRec *>(ctx->d_recs);
+    ISS_CUDA_OK(cudaMemcpyAsync(d_recs, recs.data(), sizeof(FeatRec) * (n_seq + 1), cudaMemcpyHostToDevice, st));
+    loge_tile_partials_multi_kernel<<<(unsigned)((ntiles + 127) / 128), 128, 0, st>>>(d_loge, d_recs, n_seq, ntiles,
+                                                                                      ctx->d_partials);
+    loge_stats_finalize_kernel<<<(unsigned)n_seq, 1024, 0, st>>>(ctx->d_partials, d_recs, 0, d_loge_stats);
+    ISS_CUDA_OK(cudaGetLastError());
+    iss_count_launch(2);
+    return ISS_OK;
 }

@@ -57,6 +57,89 @@ __device__ __forceinline__ bool better(double c, double best)
     return !(c <= best) && (best == best);
 }
 
+// np.mean(f32 array) is f32; + np.log(ratio) (f64) promotes to f64 (segmenter.py:70).  sg = {sum, count}.
+__device__ __forceinline__ double energy_threshold(const double *sg, double log_ratio)
+{
+    const double cnt = sg[1];
+    const float mean32 = (float)(sg[0] / cnt);          // 0/0 -> NaN like the mean of an empty slice
+    return (double)mean32 + log_ratio;
+}
+
+// emissions of step `i` of src: loge against thr (energy) or log(p) of posterior row i
+template <int K, bool ENERGY>
+__device__ __forceinline__ void load_emissions(const float *__restrict__ src, int64_t i, double thr, const VitParams &prm,
+                                               double (&e)[K])
+{
+    if (ENERGY) {
+        const bool raw = (double)src[i] > thr;          // NaN thr -> all false
+        e[0] = raw ? prm.emis_miss : prm.emis_hit;
+        e[1] = raw ? prm.emis_hit : prm.emis_miss;
+    } else {
+#pragma unroll
+        for (int j = 0; j < K; ++j)                     // np.log on float32, correctly rounded
+            e[j] = (double)(float)log((double)src[i * K + j]);
+    }
+}
+
+// one DP step on emissions `es`; `is_first` only for the very first step of the sequence.  Returns the step's
+// back-pointers, 2 bits per destination state.
+template <int K, bool ENERGY>
+__device__ __forceinline__ unsigned vit_step(double (&V)[K], const double (&es)[K], const VitParams &prm, bool is_first)
+{
+    unsigned bp = 0;
+    if (is_first) {
+#pragma unroll
+        for (int j = 0; j < K; ++j) { V[j] = es[j] + prm.prior; bp |= (unsigned)j << (2 * j); }
+    } else {
+        double Vn[K];
+#pragma unroll
+        for (int j = 0; j < K; ++j) {
+            double best = V[0] + prm.A[0][j];
+            double vn = es[j] + best;
+            unsigned arg = 0;
+#pragma unroll
+            for (int k = 1; k < K; ++k) {
+                const double c = V[k] + prm.A[k][j];
+                const double vc = es[j] + c;            // speculative: same op whichever wins
+                // energy emissions / transitions are finite constants: V can never be NaN there
+                const bool u = ENERGY ? (c > best) : better(c, best);
+                best = u ? c : best;
+                vn = u ? vc : vn;
+                arg = u ? (unsigned)k : arg;
+            }
+            Vn[j] = vn;
+            bp |= arg << (2 * j);
+        }
+#pragma unroll
+        for (int j = 0; j < K; ++j) V[j] = Vn[j];
+    }
+    return bp;
+}
+
+// first argmax (numpy.argmax, NaN rule of better())
+template <int K>
+__device__ __forceinline__ int first_argmax(const double (&V)[K])
+{
+    int arg = 0;
+    double best = V[0];
+#pragma unroll
+    for (int k = 1; k < K; ++k) {
+        const bool u = better(V[k], best);
+        best = u ? V[k] : best;
+        arg = u ? k : arg;
+    }
+    return arg;
+}
+
+// composition of back-pointer maps: (f o m)[x] = f[m[x]], 2-bit fields
+__device__ __forceinline__ unsigned compose_map(unsigned f, unsigned m)
+{
+    unsigned r = 0;
+#pragma unroll
+    for (int x = 0; x < 4; ++x) r |= ((f >> (2 * ((m >> (2 * x)) & 3))) & 3) << (2 * x);
+    return r;
+}
+
 template <int K, bool ENERGY>
 __global__ void __launch_bounds__(32)
 viterbi_forward_kernel(const float *__restrict__ src, const double *__restrict__ stats, VitParams prm, VitLayout lay)
@@ -67,14 +150,7 @@ viterbi_forward_kernel(const float *__restrict__ src, const double *__restrict__
     const int64_t T = lay.seg_off[seg + 1] - t0;
     if (T <= 0) return;
     const bool cont = lay.vin != nullptr;          // first step is an ordinary transition from vin
-    double thr = 0.0;
-    if (ENERGY) {
-        // np.mean(f32 array) is f32; + np.log(ratio) (f64) promotes to f64 (segmenter.py:70)
-        const double *sg = stats + (int64_t)seg * lay.stats_stride;
-        const double cnt = sg[1];
-        const float mean32 = (float)(sg[0] / cnt);          // 0/0 -> NaN like the mean of an empty slice
-        thr = (double)mean32 + prm.log_ratio;
-    }
+    const double thr = ENERGY ? energy_threshold(stats + (int64_t)seg * lay.stats_stride, prm.log_ratio) : 0.0;
     double V[K];
 #pragma unroll
     for (int j = 0; j < K; ++j) V[j] = cont ? lay.vin[slot * MAXK + j] : 0.0;
@@ -84,50 +160,10 @@ viterbi_forward_kernel(const float *__restrict__ src, const double *__restrict__
         double e[K];
 #pragma unroll
         for (int j = 0; j < K; ++j) e[j] = 0.0;
-        if (t < T) {
-            if (ENERGY) {
-                const bool raw = (double)src[t0 + t] > thr;     // NaN thr -> all false
-                e[0] = raw ? prm.emis_miss : prm.emis_hit;
-                e[1] = raw ? prm.emis_hit : prm.emis_miss;
-            } else {
-#pragma unroll
-                for (int j = 0; j < K; ++j)                     // np.log on float32, correctly rounded
-                    e[j] = (double)(float)log((double)src[(t0 + t) * K + j]);
-            }
-        }
+        if (t < T) load_emissions<K, ENERGY>(src, t0 + t, thr, prm, e);
         const int nstep = (int)min((int64_t)32, T - base);
         unsigned mybp = 0;
-        // one DP step on emissions `es`; `is_first` only for the very first step of the sequence
-        auto dp_step = [&](const double (&es)[K], bool is_first) -> unsigned {
-            unsigned bp = 0;
-            if (is_first) {
-#pragma unroll
-                for (int j = 0; j < K; ++j) { V[j] = es[j] + prm.prior; bp |= (unsigned)j << (2 * j); }
-            } else {
-                double Vn[K];
-#pragma unroll
-                for (int j = 0; j < K; ++j) {
-                    double best = V[0] + prm.A[0][j];
-                    double vn = es[j] + best;
-                    unsigned arg = 0;
-#pragma unroll
-                    for (int k = 1; k < K; ++k) {
-                        const double c = V[k] + prm.A[k][j];
-                        const double vc = es[j] + c;            // speculative: same op whichever wins
-                        // energy emissions / transitions are finite constants: V can never be NaN there
-                        const bool u = ENERGY ? (c > best) : better(c, best);
-                        best = u ? c : best;
-                        vn = u ? vc : vn;
-                        arg = u ? (unsigned)k : arg;
-                    }
-                    Vn[j] = vn;
-                    bp |= arg << (2 * j);
-                }
-#pragma unroll
-                for (int j = 0; j < K; ++j) V[j] = Vn[j];
-            }
-            return bp;
-        };
+        auto dp_step = [&](const double (&es)[K], bool is_first) -> unsigned { return vit_step<K, ENERGY>(V, es, prm, is_first); };
         if (nstep == 32 && (base > 0 || cont)) {
             // full block, fully unrolled: the 32 x K emission shuffles do not depend on V, so they are
             // issued ahead and only the add/compare/select chain remains on the serial critical path
@@ -151,14 +187,7 @@ viterbi_forward_kernel(const float *__restrict__ src, const double *__restrict__
         if (t < T && lay.store_bp) lay.bp[t0 + t] = (uint8_t)mybp;
     }
     if (lane == 0) {
-        int arg = 0;
-        double best = V[0];
-#pragma unroll
-        for (int k = 1; k < K; ++k) {
-            const bool u = better(V[k], best);
-            best = u ? V[k] : best;
-            arg = u ? k : arg;
-        }
+        const int arg = first_argmax<K>(V);
         if (lay.store_bp) lay.last[slot] = (uint8_t)arg;
         if (lay.vout) {
 #pragma unroll
@@ -578,4 +607,160 @@ extern "C" int iss_viterbi_segments(iss_ctx *ctx, const float *d_probs, int K, c
     ISS_CUDA_OK(cudaGetLastError());
     iss_count_launch();
     return run_backtrack(lay, hp, n_seg, 1, d_states, st);
+}
+
+// ---- online decoding of live streams (stream.py) ----------------------------------------------------------------
+// Many chains, each continued by one call from its carried scores.  A chain's undecided steps keep their back-pointer
+// bytes in its history row.  After the forward steps the chain's K end states are traced back together: the latest step
+// at which all K paths meet is the merge point m, and every state up to m is final.  Every path that ends optimally
+// later passes through one of the K states traced back from, and their back-pointers never change, so the decided
+// states are exactly those of the offline decode of the whole chain.  A chain flagged as ending is traced back in full
+// from the first argmax, as the offline backtrack does.
+namespace {
+
+struct OnlineChain {
+    int64_t src;                   // first step in d_src (energy: loge entry; CNN: posterior row)
+    int64_t n;                     // new steps
+    int64_t slot;                  // row of the scores / history / threshold tables
+    int64_t pend;                  // undecided steps already in the history row
+    int64_t out;                   // first decided state in d_out
+    int64_t flags;                 // ISS_ONLINE_START | ISS_ONLINE_END
+};
+
+template <int K, bool ENERGY>
+__global__ void __launch_bounds__(32)
+viterbi_online_kernel(const float *__restrict__ src, const double *__restrict__ stats, VitParams prm,
+                      const OnlineChain *__restrict__ chains, double *__restrict__ scores, uint8_t *__restrict__ hist,
+                      int64_t hist_cap, uint8_t *__restrict__ out, int64_t *__restrict__ ndec)
+{
+    const OnlineChain c = chains[blockIdx.x];
+    const int lane = threadIdx.x;
+    const bool start = (c.flags & 1) != 0, end = (c.flags & 2) != 0;
+    uint8_t *h = hist + c.slot * hist_cap;
+    const double thr = ENERGY ? energy_threshold(stats + 2 * c.slot, prm.log_ratio) : 0.0;
+    double V[K];
+#pragma unroll
+    for (int j = 0; j < K; ++j) V[j] = start ? 0.0 : scores[c.slot * MAXK + j];
+
+    for (int64_t base = 0; base < c.n; base += 32) {
+        const int64_t t = base + lane;
+        double e[K];
+#pragma unroll
+        for (int j = 0; j < K; ++j) e[j] = 0.0;
+        if (t < c.n) load_emissions<K, ENERGY>(src, c.src + t, thr, prm, e);
+        const int nstep = (int)min((int64_t)32, c.n - base);
+        unsigned mybp = 0;
+        for (int s = 0; s < nstep; ++s) {
+            double es[K];
+#pragma unroll
+            for (int j = 0; j < K; ++j) es[j] = __shfl_sync(0xffffffffu, e[j], s);
+            const unsigned bp = vit_step<K, ENERGY>(V, es, prm, start && base + s == 0);
+            if (lane == s) mybp = bp;
+        }
+        if (t < c.n) h[c.pend + t] = (uint8_t)mybp;
+    }
+    __syncwarp();                                      // the lanes' back-pointer stores are visible to lane 0
+
+    const int64_t P = c.pend + c.n;                    // undecided steps: h[0 .. P)
+    int64_t nd = 0;
+    if (lane == 0) {
+        int64_t m = -1;                                // last decided step
+        unsigned x = 0;
+        if (end) {
+            m = P - 1;
+            x = (unsigned)first_argmax<K>(V);
+        } else {
+            unsigned map = 0xE4;                       // end state -> state at step i (identity at i = P - 1)
+            for (int64_t i = P - 1; i >= 0; --i) {
+                bool same = true;
+#pragma unroll
+                for (int k = 1; k < K; ++k) same = same && (((map >> (2 * k)) & 3) == (map & 3));
+                if (same) { m = i; x = map & 3; break; }
+                if (i == 0) break;
+                map = compose_map(h[i], map);
+            }
+        }
+        for (int64_t r = m; r >= 0; --r) {
+            out[c.out + r] = (uint8_t)x;
+            if (r > 0) x = (h[r] >> (2 * x)) & 3;
+        }
+        nd = m + 1;
+        ndec[blockIdx.x] = nd;
+#pragma unroll
+        for (int k = 0; k < K; ++k) scores[c.slot * MAXK + k] = V[k];
+    }
+    nd = __shfl_sync(0xffffffffu, nd, 0);
+    if (end || nd == 0) return;
+    // drop the decided steps: h[nd .. P) -> h[0 .. P - nd), 32 bytes per round, reads before writes
+    for (int64_t b = 0; b < P - nd; b += 32) {
+        const int64_t i = b + lane;
+        const uint8_t v = i < P - nd ? h[nd + i] : 0;
+        __syncwarp();
+        if (i < P - nd) h[i] = v;
+        __syncwarp();
+    }
+}
+
+template <int K, bool ENERGY>
+void launch_online(int n, cudaStream_t st, const float *src, const double *stats, const VitParams &prm,
+                   const OnlineChain *chains, double *scores, uint8_t *hist, int64_t hist_cap, uint8_t *out, int64_t *ndec)
+{
+    viterbi_online_kernel<K, ENERGY><<<n, 32, 0, st>>>(src, stats, prm, chains, scores, hist, hist_cap, out, ndec);
+}
+
+}  // namespace
+
+extern "C" int64_t iss_viterbi_online_work_bytes(int n_chain)
+{
+    return n_chain < 0 ? -1 : (int64_t)sizeof(OnlineChain) * n_chain;
+}
+
+extern "C" int iss_viterbi_online(iss_ctx *ctx, int K, int n_chain, const int64_t *h_chains, const float *d_src,
+                                  int64_t src_len, const double *d_stats, double log_ratio, const double *h_emis,
+                                  const double *h_trans, double log_prior, double *d_scores, uint8_t *d_hist,
+                                  int64_t n_slots, int64_t hist_cap, uint8_t *d_out, int64_t out_len, int64_t *d_ndec,
+                                  void *d_work, void *stream)
+{
+    const bool energy = h_emis != nullptr;
+    ISS_REQUIRE(ctx && h_trans && n_chain >= 0, ISS_ERR_INVALID, "iss_viterbi_online: bad argument");
+    ISS_REQUIRE(K >= 2 && K <= MAXK && (!energy || K == 2), ISS_ERR_UNSUPPORTED, "iss_viterbi_online: K=%d not supported", K);
+    if (n_chain == 0) return ISS_OK;
+    ISS_REQUIRE(h_chains && d_scores && d_hist && d_out && d_ndec && d_work && (!energy || d_stats), ISS_ERR_INVALID,
+                "iss_viterbi_online: NULL buffer");
+    for (int i = 0; i < n_chain; ++i) {
+        const int64_t *c = h_chains + 6 * i;
+        ISS_REQUIRE(c[1] >= 0 && c[2] >= 0 && c[3] >= 0 && c[4] >= 0 && (c[1] == 0 || c[0] >= 0), ISS_ERR_INVALID,
+                    "iss_viterbi_online: chain %d: negative field", i);
+        ISS_REQUIRE(c[1] == 0 || c[0] + c[1] <= src_len, ISS_ERR_INVALID,
+                    "iss_viterbi_online: chain %d: steps %lld .. %lld outside d_src (%lld steps)", i, (long long)c[0],
+                    (long long)(c[0] + c[1]), (long long)src_len);
+        ISS_REQUIRE(c[2] < n_slots, ISS_ERR_INVALID, "iss_viterbi_online: chain %d: slot %lld of %lld", i,
+                    (long long)c[2], (long long)n_slots);
+        ISS_REQUIRE(c[4] + c[3] + c[1] <= out_len, ISS_ERR_INVALID,
+                    "iss_viterbi_online: chain %d: decided states %lld .. %lld outside d_out (%lld)", i, (long long)c[4],
+                    (long long)(c[4] + c[3] + c[1]), (long long)out_len);
+        ISS_REQUIRE(c[3] + c[1] <= hist_cap, ISS_ERR_INVALID,
+                    "iss_viterbi_online: chain %d: %lld undecided steps exceed the history capacity %lld", i,
+                    (long long)(c[3] + c[1]), (long long)hist_cap);
+        ISS_REQUIRE(!(c[5] & 1) || (c[3] == 0 && c[1] > 0), ISS_ERR_INVALID,
+                    "iss_viterbi_online: chain %d starts without steps or with a history", i);
+        ISS_REQUIRE(c[1] == 0 || d_src, ISS_ERR_INVALID, "iss_viterbi_online: NULL d_src");
+    }
+    ISS_CUDA_OK(cudaSetDevice(ctx->device));
+    cudaStream_t st = iss_stream(stream);
+    OnlineChain *d_chains = reinterpret_cast<OnlineChain *>(d_work);
+    ISS_CUDA_OK(cudaMemcpyAsync(d_chains, h_chains, sizeof(OnlineChain) * n_chain, cudaMemcpyHostToDevice, st));
+    VitParams prm = {};
+    if (energy) fill_energy_params(prm, h_emis, h_trans, log_prior, log_ratio);
+    else {
+        for (int i = 0; i < K; ++i) for (int j = 0; j < K; ++j) prm.A[i][j] = h_trans[i * K + j];
+        prm.prior = log_prior;
+    }
+    if (energy) launch_online<2, true>(n_chain, st, d_src, d_stats, prm, d_chains, d_scores, d_hist, hist_cap, d_out, d_ndec);
+    else if (K == 2) launch_online<2, false>(n_chain, st, d_src, nullptr, prm, d_chains, d_scores, d_hist, hist_cap, d_out, d_ndec);
+    else if (K == 3) launch_online<3, false>(n_chain, st, d_src, nullptr, prm, d_chains, d_scores, d_hist, hist_cap, d_out, d_ndec);
+    else launch_online<4, false>(n_chain, st, d_src, nullptr, prm, d_chains, d_scores, d_hist, hist_cap, d_out, d_ndec);
+    ISS_CUDA_OK(cudaGetLastError());
+    iss_count_launch();
+    return ISS_OK;
 }

@@ -296,3 +296,51 @@ def energy_emit(ctx, loge, end_state, out_stride=2, stream=None):
     _lib.check(lib.iss_energy_emit(ctx.handle, L, int(end_state), int(out_stride), _lib.ptr(states), _lib.ptr(work),
                                    _stream_ptr(loge.device, stream)), 'iss_energy_emit')
     return states
+
+
+# ---- live streams (stream.py) ------------------------------------------------------------------------------------
+def loge_stats_multi(ctx, loge, offs, lens, stream=None):
+    """loge_stats of each sequence loge[offs[i]:offs[i] + lens[i]] of one CUDA float32 buffer -> CUDA float64 [n, 2]."""
+    offs = np.ascontiguousarray(offs, dtype=np.int64)
+    lens = np.ascontiguousarray(lens, dtype=np.int64)
+    stats = torch.empty((len(offs), 2), dtype=torch.float64, device=loge.device)
+    _lib.check(_lib.load().iss_loge_stats_multi(ctx.handle, _lib.ptr(loge), _lib.ptr(offs), _lib.ptr(lens), len(offs),
+                                                _lib.ptr(stats), _stream_ptr(loge.device, stream)), 'iss_loge_stats_multi')
+    return stats
+
+
+ONLINE_START, ONLINE_END = 1, 2
+
+
+def viterbi_online(ctx, chains, src, scores, hist, out_len, K=2, trans=None, stats=None, energy_ratio=None, stream=None):
+    """One call of many online Viterbi chains (iss_viterbi_online).  chains: int64 [n, 6] rows {src, n, slot, pend, out,
+    flags}; src: CUDA float32 loge (energy mode: `stats` CUDA float64 [slots, 2] and `energy_ratio` given) or posteriors
+    [rows, K] (CNN mode: `trans` the K x K transition matrix); scores (CUDA float64 [slots, 4]) and hist (CUDA uint8
+    [slots, cap]) carry the chains from call to call.  Returns one CUDA uint8 buffer: n int64 decided counts, then
+    out_len decided states, so that the host reads both back in one copy."""
+    chains = np.ascontiguousarray(chains, dtype=np.int64).reshape(-1, 6)
+    n = len(chains)
+    buf = torch.empty((8 * n + max(int(out_len), 1),), dtype=torch.uint8, device=src.device)
+    if n == 0:
+        return buf
+    lib = _lib.load()
+    work = ctx.workspace('vit_online', lib.iss_viterbi_online_work_bytes(n))
+    if stats is not None:
+        t, prior, lr = _energy_consts(energy_ratio)
+        emis, K = _EMIS, 2
+    else:
+        t, prior, lr, emis = np.ascontiguousarray(trans, dtype=np.float64), float(np.log(np.ones(K) / K)[0]), 0.0, None
+    n_slots = min(scores.shape[0], hist.shape[0], stats.shape[0] if stats is not None else scores.shape[0])
+    _lib.check(lib.iss_viterbi_online(ctx.handle, int(K), n, _lib.ptr(chains), _lib.ptr(src), src.shape[0],
+                                      _lib.ptr(stats), lr, _lib.ptr(emis), _lib.ptr(t), prior, _lib.ptr(scores),
+                                      _lib.ptr(hist), n_slots, hist.shape[1],
+                                      _lib.ptr(buf[8 * n:]), buf.numel() - 8 * n,
+                                      _lib.ptr(buf[:8 * n].view(torch.int64)), _lib.ptr(work),
+                                      _stream_ptr(src.device, stream)), 'iss_viterbi_online')
+    return buf
+
+
+def split_online(host_buf, n):
+    """(decided counts int64 [n], decided states uint8) of a viterbi_online buffer copied to the host."""
+    host_buf = np.asarray(host_buf)
+    return host_buf[:8 * n].view(np.int64), host_buf[8 * n:]

@@ -377,6 +377,13 @@ class Segmenter:
         return [[(lab, start_sec + start * .02, start_sec + stop * .02) for lab, start, stop in lseg]
                 for lseg, start_sec in zip(lsegs, start_secs)]
 
+    def stream(self, calibration_sec=60.0):
+        """Extension: live segmentation of many 16 kHz mono streams fed chunk by chunk (``stream.LiveStreams``).  The
+        energy threshold of a stream comes from its first ``calibration_sec`` seconds (>= 1); no label is decided
+        before that."""
+        from .stream import LiveStreams
+        return LiveStreams(self, calibration_sec)
+
     def batch_process(self, linput, loutput, verbose=False, skipifexist=False, nbtry=1, trydelay=2., output_format='csv'):
         """segmenter.py:297-335 -- same return tuple and message codes."""
         if verbose:

@@ -39,7 +39,7 @@ typedef struct iss_mlp iss_mlp;
 
 /* ---- library / context ------------------------------------------------- */
 
-#define ISS_ABI_VERSION 5
+#define ISS_ABI_VERSION 6
 int         iss_version(void);               /* == ISS_ABI_VERSION of the header the library was built from */
 const char *iss_last_error(void);
 /* Creates a context bound to CUDA device `device` (one per host thread that
@@ -109,6 +109,11 @@ int iss_sidekit_features_multi(iss_ctx *ctx, int n_rec, const void *const *h_pcm
  * order as the fused reduction inside iss_sidekit_features, hence bit-identical
  * d_loge_stats for the same loge values. */
 int iss_loge_stats(iss_ctx *ctx, const float *d_loge, int64_t L, double *d_loge_stats, void *stream);
+/* iss_loge_stats on each of n_seq sequences of one buffer in one pass: sequence i is d_loge[h_loge_off[i] ..
+ * + h_len[i]) (h_len[i] >= 1), its {sum, count} goes to d_loge_stats[2i ..].  Bit-identical to iss_loge_stats on
+ * the sequence alone.  Live streams use it for the calibration prefixes of their energy thresholds. */
+int iss_loge_stats_multi(iss_ctx *ctx, const float *d_loge, const int64_t *h_loge_off, const int64_t *h_len,
+                         int n_seq, double *d_loge_stats, void *stream);
 
 /* ---- K3: Viterbi smoothing ------------------------------------------------
  * Replaces viterbi_decoding(emission, transition) for the two ways the hot
@@ -155,6 +160,31 @@ int iss_viterbi_segments(iss_ctx *ctx, const float *d_probs, int K, const int64_
                          int n_seg, const double *h_trans, double log_prior, uint8_t *d_states,
                          void *d_work, void *stream);
 int64_t iss_viterbi_work_bytes(int64_t total_steps, int n_seg);
+
+/* Online decoding of many Viterbi chains in one launch (live streams: inaspeechsegmenter_b200/stream.py).  Chain i
+ * is h_chains[6i .. 6i+6) = {src, n, slot, pend, out, flags} (int64, host):
+ *   - its n new steps are d_src entries src .. src+n: energy mode (h_emis != NULL, K == 2) thresholds loge against
+ *     the threshold of iss_energy_viterbi from d_stats[2*slot ..]; CNN mode (h_emis == NULL) takes log(p) of the
+ *     posterior rows d_src[(src+t)*K ..];
+ *   - flags & ISS_ONLINE_START: the chain starts here (V = E + log_prior on its first step, pend must be 0);
+ *     otherwise it continues from the scores d_scores[slot*4 .. +K) left by its previous call;
+ *   - the back-pointers of its pend undecided steps are d_hist[slot*hist_cap ..]; the new steps' are appended
+ *     (pend + n <= hist_cap);
+ *   - every state up to the latest step at which the backtracks from all K end states meet is final; with
+ *     flags & ISS_ONLINE_END the chain ends and all its states are final (backtrack from the first argmax).
+ * The decided states (one byte each, oldest first) go to d_out[out ..], their count to d_ndec[i]; the history row
+ * keeps only the still undecided steps.  Same arithmetic as iss_energy_viterbi / iss_viterbi_segments, so the
+ * decided states of a chain are those of the offline decode of all its steps.  d_scores, d_hist and d_stats are
+ * caller-owned and live across calls; d_work holds iss_viterbi_online_work_bytes(n_chain) bytes.  Sizes, checked
+ * against every chain before the launch: d_src holds src_len steps (entries or rows), d_scores / d_hist / d_stats
+ * n_slots slots, d_out out_len bytes (chain i needs out + pend + n of them). */
+#define ISS_ONLINE_START 1
+#define ISS_ONLINE_END   2
+int iss_viterbi_online(iss_ctx *ctx, int K, int n_chain, const int64_t *h_chains, const float *d_src,
+                       int64_t src_len, const double *d_stats, double log_ratio, const double *h_emis,
+                       const double *h_trans, double log_prior, double *d_scores, uint8_t *d_hist, int64_t n_slots,
+                       int64_t hist_cap, uint8_t *d_out, int64_t out_len, int64_t *d_ndec, void *d_work, void *stream);
+int64_t iss_viterbi_online_work_bytes(int n_chain);
 
 /* Partial chains of the energy Viterbi for a recording that is time-sharded across GPUs
  * (the whole-file chain of pyannote_viterbi.py:202-220 cut at rank boundaries):
