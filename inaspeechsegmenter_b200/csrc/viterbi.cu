@@ -76,8 +76,8 @@ __device__ __forceinline__ void load_emissions(const float *__restrict__ src, in
         e[1] = raw ? prm.emis_hit : prm.emis_miss;
     } else {
 #pragma unroll
-        for (int j = 0; j < K; ++j)                     // np.log on float32, correctly rounded
-            e[j] = (double)(float)log((double)src[i * K + j]);
+        for (int j = 0; j < K; ++j)                     // float32(log(double p)): a correctly rounded float32 log.
+            e[j] = (double)(float)log((double)src[i * K + j]);   // numpy's float32 log is not (DESIGN, "Emission log")
     }
 }
 
@@ -439,7 +439,7 @@ extern "C" int iss_energy_emit(iss_ctx *ctx, int64_t L, int end_state, int out_s
 // (one addition of a chunk-relative score instead of ECH stepwise additions), which could only matter for a
 // path tie closer than ~1e-8 -- the path scores are sums of a handful of constants (-5, -345.39, -23.03, -1e-10)
 // whose distinct combinations are orders of magnitude further apart.  The serial kernel stays available
-// (ISS_B200_VITERBI=serial, and it is what the GPU tests compare this against on 10 h tracks).
+// (ISS_B200_VITERBI=serial); the GPU tests compare both with the C oracle, 10 h tracks included.
 constexpr int64_t ECH = 16384;
 
 __global__ void energy_entry_compose_kernel(const double *__restrict__ v0, const double *__restrict__ basis_out,

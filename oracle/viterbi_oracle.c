@@ -34,19 +34,32 @@ static int argmax_first(const double *v, int n)
     return best;
 }
 
-/* emission: [T,K] row-major doubles; trans: [K,K] (from,to); states: [T] out.
- * scratch for back-pointers is allocated here. returns 0 on success. */
-int oracle_viterbi(const double *emission, const double *trans, int64_t T, int K,
-                   int32_t *states)
+/* A partial chain: the same DP on steps [0, T) of a longer chain, in the same order of double operations.
+ *   vin       [K] scores V[-1] of the step before the first, or NULL.  With vin the first step is an ordinary
+ *             transition from it; without, V[0] = E[0] + log(1/K).
+ *   vout      [K] out: V[T-1] (or NULL).
+ *   backmap   [K] out: for each end state x, the state the path ending in x has before the first step (with vin)
+ *             or at the first step (without); NULL to skip.
+ *   end_state -1: backtrack from the first argmax of V[T-1]; else from that state.
+ *   states    out: X[t] for every t % out_stride == 0, at states[t / out_stride] (or NULL).
+ * Returns 0 on success. */
+int oracle_viterbi_partial(const double *emission, const double *trans, int64_t T, int K, const double *vin,
+                           double *vout, int32_t *backmap, int end_state, int out_stride, int32_t *states)
 {
-    if (K < 1 || K > ORACLE_MAXK || T < 1) return -1;
+    if (K < 1 || K > ORACLE_MAXK || T < 1 || out_stride < 1 || end_state < -1 || end_state >= K) return -1;
     uint8_t *bp = (uint8_t *)malloc((size_t)T * (size_t)K);
     if (!bp) return -2;
     double V[ORACLE_MAXK], Vn[ORACLE_MAXK], cand[ORACLE_MAXK];
-    /* np.log(np.ones(k) / k) */
-    const double prior = log(1.0 / (double)K);
-    for (int j = 0; j < K; ++j) { V[j] = emission[j] + prior; bp[j] = (uint8_t)j; }
-    for (int64_t t = 1; t < T; ++t) {
+    int64_t t = 0;
+    if (!vin) {
+        /* np.log(np.ones(k) / k) */
+        const double prior = log(1.0 / (double)K);
+        for (int j = 0; j < K; ++j) { V[j] = emission[j] + prior; bp[j] = (uint8_t)j; }
+        t = 1;
+    } else {
+        for (int j = 0; j < K; ++j) V[j] = vin[j];
+    }
+    for (; t < T; ++t) {
         const double *e = emission + t * K;
         for (int j = 0; j < K; ++j) {
             for (int k = 0; k < K; ++k) cand[k] = V[k] + trans[k * K + j];
@@ -56,14 +69,31 @@ int oracle_viterbi(const double *emission, const double *trans, int64_t T, int K
         }
         for (int j = 0; j < K; ++j) V[j] = Vn[j];
     }
-    int x = argmax_first(V, K);
-    states[T - 1] = x;
-    for (int64_t t = T - 1; t >= 1; --t) {
-        x = bp[t * K + x];
-        states[t - 1] = x;
+    if (vout) for (int j = 0; j < K; ++j) vout[j] = V[j];
+    if (backmap) {
+        for (int x0 = 0; x0 < K; ++x0) {
+            int x = x0;
+            for (int64_t s = T - 1; s >= (vin ? 0 : 1); --s) x = bp[s * K + x];
+            backmap[x0] = x;
+        }
+    }
+    if (states) {
+        int x = end_state >= 0 ? end_state : argmax_first(V, K);
+        for (int64_t s = T - 1; s >= 0; --s) {
+            if (s % out_stride == 0) states[s / out_stride] = x;
+            if (s > 0) x = bp[s * K + x];
+        }
     }
     free(bp);
     return 0;
+}
+
+/* emission: [T,K] row-major doubles; trans: [K,K] (from,to); states: [T] out.
+ * scratch for back-pointers is allocated here. returns 0 on success. */
+int oracle_viterbi(const double *emission, const double *trans, int64_t T, int K,
+                   int32_t *states)
+{
+    return oracle_viterbi_partial(emission, trans, T, K, NULL, NULL, NULL, -1, 1, states);
 }
 
 /* float32 emissions (np.log(r) of a float32 softmax, segmenter.py:176):

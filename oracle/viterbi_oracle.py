@@ -8,6 +8,10 @@ Two implementations of the same order of floating-point operations:
 ``viterbi_numpy`` (pure numpy/Python loop, small cases) and ``viterbi_c``
 (``viterbi_oracle.c`` through ctypes, long sequences).  Both are pinned
 against the real ``viterbi_decoding`` by ``tests/golden/make_golden.py``.
+``viterbi_partial`` runs a cut of a longer chain (incoming scores, outgoing
+scores, back-map, forced end state, output stride) in the same order of
+operations; ``emissions_kernel`` and ``energy_threshold_kernel`` are the CUDA
+kernels' own emission and threshold, for the exact GPU comparisons.
 """
 import ctypes
 import os
@@ -35,6 +39,10 @@ def _lib():
             fn.restype = ctypes.c_int
             fn.argtypes = [ctypes.POINTER(etype), ctypes.POINTER(ctypes.c_double),
                            ctypes.c_int64, ctypes.c_int, ctypes.POINTER(ctypes.c_int32)]
+        lib.oracle_viterbi_partial.restype = ctypes.c_int
+        lib.oracle_viterbi_partial.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_int,
+                                               ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int,
+                                               ctypes.c_int, ctypes.c_void_p]
         _LIB = lib
     return _LIB
 
@@ -105,6 +113,68 @@ def viterbi_c(emission, transition):
     if rc != 0:
         raise RuntimeError('oracle_viterbi failed rc=%d' % rc)
     return out.astype(np.float64)
+
+
+def viterbi_partial(emission, transition, vin=None, end_state=-1, out_stride=1):
+    """Steps [0, T) of a longer chain (``oracle_viterbi_partial``): with ``vin`` (V of the step before) the first
+    step is an ordinary transition, without it the prior log(1/K) applies.  Returns (states int32 [ceil(T /
+    out_stride)], vout float64 [K] = V[T-1], backmap int32 [K]: for each end state, the state before the first step
+    (with vin) or at the first step (without)).  ``end_state`` -1 backtracks from the first argmax of V[T-1]."""
+    em = np.ascontiguousarray(emission, dtype=np.float64)
+    T, K = em.shape
+    trans = np.ascontiguousarray(transition, dtype=np.float64)
+    states = np.empty((T + out_stride - 1) // out_stride, dtype=np.int32)
+    vout = np.empty(K, dtype=np.float64)
+    bmap = np.empty(K, dtype=np.int32)
+    vin_arr = None if vin is None else np.ascontiguousarray(vin, dtype=np.float64)
+    rc = _lib().oracle_viterbi_partial(em.ctypes.data, trans.ctypes.data, T, K,
+                                       None if vin_arr is None else vin_arr.ctypes.data, vout.ctypes.data,
+                                       bmap.ctypes.data, int(end_state), int(out_stride), states.ctypes.data)
+    if rc != 0:
+        raise RuntimeError('oracle_viterbi_partial failed rc=%d' % rc)
+    return states, vout, bmap
+
+
+# ---- emissions and thresholds as the CUDA kernels define them ---------------------------------
+
+def emissions_kernel(p):
+    """The K3 kernels' emission: float32(log(float64(p))), a correctly rounded float32 log, widened to double.
+    numpy's float32 ``np.log`` (what the reference applies, segmenter.py:176) is not correctly rounded; this is the
+    definition the GPU comparisons use, so they do not depend on the host's SIMD log."""
+    with np.errstate(divide='ignore'):
+        return np.log(np.asarray(p, dtype=np.float32).astype(np.float64)).astype(np.float32).astype(np.float64)
+
+
+def f32_midpoint_margin(p):
+    """Distance of log(float64(p)) from the nearest float32 rounding midpoint, in float64 ulps of the log (inf for
+    p = 0 or 1).  A value within a few ulps could round to a different float32 in another double log (CUDA's or the
+    host's), so fixtures assert a margin."""
+    with np.errstate(divide='ignore'):
+        d = np.log(np.asarray(p, dtype=np.float32).astype(np.float64))
+    f = d.astype(np.float32).astype(np.float64)
+    up = np.nextafter(d.astype(np.float32), np.float32(np.inf)).astype(np.float64)
+    dn = np.nextafter(d.astype(np.float32), np.float32(-np.inf)).astype(np.float64)
+    other = np.where(f <= d, up, dn)
+    mid = 0.5 * (f + other)                          # exact: float32 neighbours need 25 bits
+    with np.errstate(invalid='ignore'):
+        m = np.abs(d - mid) / np.spacing(np.abs(d))
+    return np.where(np.isfinite(d) & (d != 0), m, np.inf)
+
+
+def energy_threshold_kernel(stats, ratio):
+    """The K3 kernels' energy threshold from the ``loge_stats`` pair {sum, count}: float32(sum / count) + log(ratio)
+    (NaN for an all-silent track)."""
+    s, c = float(stats[0]), float(stats[1])
+    with np.errstate(invalid='ignore', divide='ignore'):
+        mean = np.float32(np.float64(s) / np.float64(c))
+    return float(np.float64(mean) + np.log(ratio))
+
+
+def energy_activity_thr(loge, thr):
+    """segmenter.py:69-73 from a given threshold: ``loge > thr`` (float64 compare; a NaN threshold marks nothing
+    active), then the 2-state Viterbi with the energy transitions.  int32 states."""
+    raw = np.asarray(loge, dtype=np.float32).astype(np.float64) > thr
+    return viterbi_partial(pred2logemission(raw), log_trans_exp(150, cost0=-5))[0]
 
 
 def viterbi_decoding(emission, transition):
