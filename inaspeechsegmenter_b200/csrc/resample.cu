@@ -9,10 +9,15 @@
 // The host designs h (resample.py); iss_resample_upload_taps arranges it by phase: output k, with
 // k * down = a * up + q, needs the taps of phase q against the frames a + s_q .. a + s_q + n_q - 1, ascending.
 //
-// Layout: one CTA owns a tile of consecutive outputs of one recording (tiles start at the recording's first output).
+// Layout: one CTA owns a tile of consecutive outputs of one record (tiles start at the record's first output k_first).
 // It stages the raw samples of the tile's input span in shared memory with 16-byte loads (scalar loads when the
-// recording's base pointer is not 16-byte aligned), downmixes them there into float64, then each thread evaluates
+// record's base pointer is not 16-byte aligned), downmixes them there into float64, then each thread evaluates
 // its outputs as float64 FMA chains in ascending frame order.  No atomics, and no value depends on the tiling.
+//
+// Windows (live streams): a record's buffer holds frames [f_base, n_known) of its stream, and it computes outputs
+// [k_first, k_first + n_out).  Frames at or past n_known read as zero, as do frames before 0.  A whole recording is
+// the window f_base = 0, k_first = 0, n_out = ceil(n * up / down); iss_resample_window_multi checks on the host that
+// no output of a window reads a frame in [0, f_base), and that only a stream's final outputs read past n_known.
 #include <math.h>
 #include <string.h>
 
@@ -37,12 +42,15 @@ struct Phase {
     int pad;
 };
 
-// One recording of a resampling call.  Its tiles are [tile_off, next recording's tile_off).
+// One record (a recording, or a window of a stream) of a resampling call.  Its tiles are [tile_off, next record's
+// tile_off).
 struct RsRec {
-    const void *pcm;
-    int64_t n_frames;
+    const void *pcm;                // frame f_base of the stream
+    int64_t f_base;
+    int64_t n_known;                // frames >= n_known are zero
+    int64_t k_first;
     int64_t n_out;
-    int64_t out_off;                // first int16 output element
+    int64_t out_off;                // int16 element of output k_first
     int64_t tile_off;               // first tile (global block index); entry n_rec holds the total
     int vec_ok;                     // pcm is 16-byte aligned
 };
@@ -64,18 +72,18 @@ resample_kernel(const RsRec *__restrict__ recs, int n_rec, const Phase *__restri
     while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (recs[mid].tile_off <= (int64_t)blockIdx.x) lo = mid; else hi = mid; }
     const RsRec &rec = recs[lo];
     const Sample *pcm = reinterpret_cast<const Sample *>(rec.pcm);
-    const int64_t n = rec.n_frames;
-    const int64_t k0 = ((int64_t)blockIdx.x - rec.tile_off) * tile_out;
-    const int nk = (int)min((int64_t)tile_out, rec.n_out - k0);
+    const int64_t fb = rec.f_base, n = rec.n_known;
+    const int64_t k0 = rec.k_first + ((int64_t)blockIdx.x - rec.tile_off) * tile_out;
+    const int nk = (int)min((int64_t)tile_out, rec.k_first + rec.n_out - k0);
     const int64_t f_lo = (k0 * down) / up + s_min;                            // input frames [f_lo, f_hi)
     const int64_t f_hi = ((k0 + nk - 1) * down) / up + e_max;
     const int span = (int)(f_hi - f_lo);                                      // <= span_cap
 
-    // ---- raw samples of frames [max(f_lo, 0), min(f_hi, n)) ----
-    const int64_t g_lo = max(f_lo, (int64_t)0), g_hi = min(f_hi, n);
-    int64_t rb = 0;                                              // raw[i] holds sample element rb + i
+    // ---- raw samples of frames [max(f_lo, f_base), min(f_hi, n)) ----
+    const int64_t g_lo = max(f_lo, fb), g_hi = min(f_hi, n);
+    int64_t rb = 0;                                              // raw[i] holds sample element rb + i of pcm
     if (g_lo < g_hi) {
-        const int64_t e_lo = g_lo * channels, e_hi = g_hi * channels;
+        const int64_t e_lo = (g_lo - fb) * channels, e_hi = (g_hi - fb) * channels;
         if (rec.vec_ok) {
             rb = e_lo & ~(int64_t)(VEC - 1);
             const int64_t v_hi = e_hi & ~(int64_t)(VEC - 1);
@@ -96,8 +104,8 @@ resample_kernel(const RsRec *__restrict__ recs, int n_rec, const Phase *__restri
     for (int i = tid; i < span; i += RS_THREADS) {
         const int64_t f = f_lo + i;
         double v = 0.0;
-        if (f >= 0 && f < n) {
-            const Sample *p = raw + (f * channels - rb);
+        if (f >= fb && f < n) {
+            const Sample *p = raw + ((f - fb) * channels - rb);
             double s = 0.0;
             for (int c = 0; c < channels; ++c) s += (double)p[c] * inv;
             v = s / (double)channels;
@@ -119,7 +127,7 @@ resample_kernel(const RsRec *__restrict__ recs, int n_rec, const Phase *__restri
         double acc = 0.0;
         for (int i = 0; i < ph.n; ++i) acc = fma(__ldg(t + i), x[i], acc);
         const double v = fmin(fmax(rint(acc * 32768.0), -32768.0), 32767.0);     // round half to even, saturate
-        out[k] = (int16_t)(int)v;
+        out[k - rec.k_first] = (int16_t)(int)v;
     }
 }
 
@@ -135,6 +143,7 @@ struct ResampleTable {
     int s_min, e_max;               // min s_q, max s_q + n_q over the phases
     Phase *d_phases;
     double *d_taps;
+    std::vector<Phase> phases;      // host copy, for the window checks
 };
 
 struct ResampleState {
@@ -204,7 +213,7 @@ extern "C" int iss_resample_upload_taps(iss_ctx *ctx, int rate, const double *h_
     ResampleState *s = rs_state(ctx);
     auto it = s->tables.find(rate);
     if (it != s->tables.end()) { free_table(it->second); s->tables.erase(it); }
-    ResampleTable t{up, down, s_min, e_max, nullptr, nullptr};
+    ResampleTable t{up, down, s_min, e_max, nullptr, nullptr, ph};
     cudaError_t e = cudaMalloc(&t.d_phases, sizeof(Phase) * ph.size());
     if (e == cudaSuccess) e = cudaMalloc(&t.d_taps, sizeof(double) * taps.size());
     if (e == cudaSuccess) e = cudaMemcpy(t.d_phases, ph.data(), sizeof(Phase) * ph.size(), cudaMemcpyHostToDevice);
@@ -256,46 +265,46 @@ static int launch_resample(const ResampleTable &t, const RsRec *d_recs, int n_re
     return ISS_OK;
 }
 
-extern "C" int iss_resample_to16k_multi(iss_ctx *ctx, int n_rec, const void *const *h_pcm, const int64_t *h_n_frames,
-                                        int channels, int rate, int pcm_format, int16_t *d_out, const int64_t *h_out_off,
-                                        void *stream)
+// Checks the common arguments of a resampling call; *out is the table of `rate`.
+static int check_call(iss_ctx *ctx, const char *fn, int n_rec, const void *args, int channels, int rate, int pcm_format,
+                      const ResampleTable **out)
 {
-    ISS_REQUIRE(ctx, ISS_ERR_INVALID, "iss_resample_to16k_multi: ctx is NULL");
+    ISS_REQUIRE(ctx, ISS_ERR_INVALID, "%s: ctx is NULL", fn);
     ISS_REQUIRE(pcm_format == ISS_PCM_F32 || pcm_format == ISS_PCM_S16, ISS_ERR_INVALID, "bad pcm_format %d", pcm_format);
     ISS_REQUIRE(channels >= 1 && channels <= RS_MAX_CHANNELS, ISS_ERR_INVALID,
-                "iss_resample_to16k_multi: %d channels outside [1, %d]", channels, RS_MAX_CHANNELS);
-    ISS_REQUIRE(rate_ok(rate), ISS_ERR_INVALID, "iss_resample_to16k_multi: rate %d outside [%d, %d]", rate, RS_MIN_RATE, RS_MAX_RATE);
-    ISS_REQUIRE(n_rec >= 1 && h_pcm && h_n_frames && h_out_off, ISS_ERR_INVALID, "iss_resample_to16k_multi: bad argument");
+                "%s: %d channels outside [1, %d]", fn, channels, RS_MAX_CHANNELS);
+    ISS_REQUIRE(rate_ok(rate), ISS_ERR_INVALID, "%s: rate %d outside [%d, %d]", fn, rate, RS_MIN_RATE, RS_MAX_RATE);
+    ISS_REQUIRE(n_rec >= 1 && args, ISS_ERR_INVALID, "%s: bad argument", fn);
     ResampleState *s = rs_state(ctx);
     auto it = s->tables.find(rate);
-    ISS_REQUIRE(it != s->tables.end(), ISS_ERR_STATE, "iss_resample_to16k_multi: no taps uploaded for rate %d", rate);
-    const ResampleTable &t = it->second;
+    ISS_REQUIRE(it != s->tables.end(), ISS_ERR_STATE, "%s: no taps uploaded for rate %d", fn, rate);
+    *out = &it->second;
+    return ISS_OK;
+}
+
+// Tiles the records (recs[0 .. n_rec), pcm .. out_off set), uploads the record table and launches.
+static int run_records(iss_ctx *ctx, const char *fn, const ResampleTable &t, std::vector<RsRec> &recs, int channels,
+                       int pcm_format, int16_t *d_out, void *stream)
+{
+    ResampleState *s = rs_state(ctx);
     ISS_CUDA_OK(cudaSetDevice(ctx->device));
     cudaStream_t st = iss_stream(stream);
     const int itemsize = pcm_format == ISS_PCM_S16 ? 2 : 4;
     int tile, span_cap;
     size_t smem;
     tile_for(t, channels, itemsize, &tile, &span_cap, &smem);
-    std::vector<RsRec> recs(n_rec + 1);
+    const int n_rec = (int)recs.size() - 1;
     int64_t ntiles = 0;
     for (int i = 0; i < n_rec; ++i) {
         RsRec &r = recs[i];
-        r.pcm = h_pcm[i];
-        r.n_frames = h_n_frames[i];
-        ISS_REQUIRE(r.n_frames >= 0 && r.n_frames < ((int64_t)1 << 40), ISS_ERR_INVALID,
-                    "iss_resample_to16k_multi: bad frame count (recording %d)", i);
-        r.n_out = iss_resample_num_frames(r.n_frames, rate);
-        r.out_off = h_out_off[i];
         r.tile_off = ntiles;
         r.vec_ok = ((reinterpret_cast<uintptr_t>(r.pcm) & 15) == 0) ? 1 : 0;
-        ISS_REQUIRE(r.n_out == 0 || r.pcm, ISS_ERR_INVALID, "iss_resample_to16k_multi: NULL buffer (recording %d)", i);
-        ISS_REQUIRE(r.out_off >= 0, ISS_ERR_INVALID, "iss_resample_to16k_multi: negative offset (recording %d)", i);
         ntiles += (r.n_out + tile - 1) / tile;
     }
-    recs[n_rec] = RsRec{nullptr, 0, 0, 0, ntiles, 0};
+    recs[n_rec] = RsRec{nullptr, 0, 0, 0, 0, 0, ntiles, 0};
     if (ntiles == 0) return ISS_OK;
-    ISS_REQUIRE(d_out, ISS_ERR_INVALID, "iss_resample_to16k_multi: NULL output");
-    ISS_REQUIRE(ntiles < (1ll << 31), ISS_ERR_INVALID, "iss_resample_to16k_multi: input too long for one call");
+    ISS_REQUIRE(d_out, ISS_ERR_INVALID, "%s: NULL output", fn);
+    ISS_REQUIRE(ntiles < (1ll << 31), ISS_ERR_INVALID, "%s: input too long for one call", fn);
     if (n_rec + 1 > s->recs_cap) {
         if (s->d_recs) ISS_CUDA_OK(cudaFree(s->d_recs));
         s->d_recs = nullptr; s->recs_cap = 0;
@@ -309,4 +318,70 @@ extern "C" int iss_resample_to16k_multi(iss_ctx *ctx, int n_rec, const void *con
     return pcm_format == ISS_PCM_S16
                ? launch_resample<ISS_PCM_S16>(t, d_recs, n_rec, ntiles, channels, tile, span_cap, smem, d_out, st)
                : launch_resample<ISS_PCM_F32>(t, d_recs, n_rec, ntiles, channels, tile, span_cap, smem, d_out, st);
+}
+
+extern "C" int iss_resample_to16k_multi(iss_ctx *ctx, int n_rec, const void *const *h_pcm, const int64_t *h_n_frames,
+                                        int channels, int rate, int pcm_format, int16_t *d_out, const int64_t *h_out_off,
+                                        void *stream)
+{
+    const char *fn = "iss_resample_to16k_multi";
+    const ResampleTable *t = nullptr;
+    const int rc = check_call(ctx, fn, n_rec, h_pcm && h_n_frames && h_out_off ? h_pcm : nullptr, channels, rate,
+                              pcm_format, &t);
+    if (rc != ISS_OK) return rc;
+    std::vector<RsRec> recs(n_rec + 1);
+    for (int i = 0; i < n_rec; ++i) {
+        RsRec &r = recs[i];
+        r.pcm = h_pcm[i];
+        r.f_base = 0;
+        r.n_known = h_n_frames[i];
+        ISS_REQUIRE(r.n_known >= 0 && r.n_known < ((int64_t)1 << 40), ISS_ERR_INVALID,
+                    "iss_resample_to16k_multi: bad frame count (recording %d)", i);
+        r.k_first = 0;
+        r.n_out = iss_resample_num_frames(r.n_known, rate);
+        r.out_off = h_out_off[i];
+        ISS_REQUIRE(r.n_out == 0 || r.pcm, ISS_ERR_INVALID, "iss_resample_to16k_multi: NULL buffer (recording %d)", i);
+        ISS_REQUIRE(r.out_off >= 0, ISS_ERR_INVALID, "iss_resample_to16k_multi: negative offset (recording %d)", i);
+    }
+    return run_records(ctx, fn, *t, recs, channels, pcm_format, d_out, stream);
+}
+
+extern "C" int iss_resample_window_multi(iss_ctx *ctx, int n_rec, const void *const *h_pcm, const int64_t *h_win,
+                                         int channels, int rate, int pcm_format, int16_t *d_out, void *stream)
+{
+    const char *fn = "iss_resample_window_multi";
+    const ResampleTable *t = nullptr;
+    const int rc = check_call(ctx, fn, n_rec, h_pcm && h_win ? h_pcm : nullptr, channels, rate, pcm_format, &t);
+    if (rc != ISS_OK) return rc;
+    const int64_t up = t->up, down = t->down;
+    std::vector<RsRec> recs(n_rec + 1);
+    for (int i = 0; i < n_rec; ++i) {
+        const int64_t *w = h_win + (size_t)i * 6;
+        const int64_t f_base = w[0], n_known = w[1], k_first = w[2], n_out = w[3], out_off = w[4], flags = w[5];
+        ISS_REQUIRE(f_base >= 0 && f_base <= n_known && n_known < ((int64_t)1 << 40) && k_first >= 0 &&
+                    k_first < ((int64_t)1 << 44) && n_out >= 0 && n_out < ((int64_t)1 << 44) && out_off >= 0 && (flags & ~(int64_t)ISS_RESAMPLE_END) == 0, ISS_ERR_INVALID,
+                    "%s: record %d: bad field", fn, i);
+        ISS_REQUIRE(k_first + n_out <= iss_resample_num_frames(n_known, rate), ISS_ERR_INVALID,
+                    "%s: record %d: outputs [%lld, %lld) past the %lld outputs of %lld frames", fn, i,
+                    (long long)k_first, (long long)(k_first + n_out), (long long)iss_resample_num_frames(n_known, rate),
+                    (long long)n_known);
+        ISS_REQUIRE(n_out == 0 || h_pcm[i], ISS_ERR_INVALID, "%s: record %d: NULL buffer", fn, i);
+        if (n_out > 0) {
+            // the frames an output reads, a + s_q .. a + s_q + n_q - 1, move forward with k: the first and last
+            // output bound the window
+            const int64_t k_last = k_first + n_out - 1;
+            const int64_t a0 = k_first * down / up, a1 = k_last * down / up;
+            const Phase &p0 = t->phases[(size_t)(k_first * down - a0 * up)];
+            const Phase &p1 = t->phases[(size_t)(k_last * down - a1 * up)];
+            const int64_t first = a0 + p0.s, last = a1 + p1.s + p1.n - 1;
+            ISS_REQUIRE(f_base == 0 || first >= f_base, ISS_ERR_INVALID,
+                        "%s: record %d: output %lld reads frame %lld, before the window's first frame %lld", fn, i,
+                        (long long)k_first, (long long)first, (long long)f_base);
+            ISS_REQUIRE((flags & ISS_RESAMPLE_END) || last < n_known, ISS_ERR_INVALID,
+                        "%s: record %d: output %lld reads frame %lld of %lld known frames, and the stream has not ended",
+                        fn, i, (long long)k_last, (long long)last, (long long)n_known);
+        }
+        recs[i] = RsRec{h_pcm[i], f_base, n_known, k_first, n_out, out_off, 0, 0};
+    }
+    return run_records(ctx, fn, *t, recs, channels, pcm_format, d_out, stream);
 }

@@ -50,6 +50,40 @@ def num_frames(n, rate):
 
 
 @functools.lru_cache(maxsize=None)
+def reach(rate):
+    """(s_min, e_max) of `rate`: output k, with k * down = a * up + q, reads the frames a + s_q .. a + s_q + n_q - 1; s_min
+    is the least s_q and e_max the largest s_q + n_q over the phases (the phase table of iss_resample_upload_taps)."""
+    up, down = factors(rate)
+    half = 0 if up == down == 1 else 10 * max(up, down)
+    b, r = divmod(half, up)
+    q = np.arange(up)
+    carry = (q + r >= up).astype(np.int64)
+    nq = (2 * half - (q + r - carry * up)) // up + 1
+    s = b + carry - (nq - 1)
+    return int(s.min()), int((s + nq).max())
+
+
+# Live streams (stream.py) resample chunk by chunk: a stream's outputs are computed once the frames they read have
+# arrived, from a window of its input that starts at its first frame still needed, and are the outputs of the whole
+# stream bit for bit (iss_resample_window_multi).  These three functions are the whole rule.
+def ready_outputs(n, rate):
+    """Outputs final once n frames have arrived: every k with floor(k * down / up) + e_max - 1 <= n - 1."""
+    return min(num_frames(max(n - reach(rate)[1] + 1, 0), rate), num_frames(n, rate))
+
+
+def end_outputs(n, rate):
+    """Outputs of a stream that ended after n frames (the last ones read the zeros past its end)."""
+    return num_frames(n, rate)
+
+
+def first_kept(k_next, rate):
+    """First input frame any output from k_next on reads (0 while that is before the stream): the start of a
+    stream's retained tail once its outputs below k_next are computed."""
+    up, down = factors(rate)
+    return max(k_next * down // up + reach(rate)[0], 0)
+
+
+@functools.lru_cache(maxsize=None)
 def lowpass(up, down):
     """float64 taps of resample_poly's default filter, ``firwin(2 * 10 * M + 1, 1 / M, window=('kaiser', 5.0)) * up``
     with M = max(up, down); the single tap 1 when up == down == 1 (resample_poly then returns its input)."""
@@ -152,6 +186,24 @@ def to16k_multi(ctx, pcms, rate, out, out_off, stream=None):
     _lib.check(_lib.load().iss_resample_to16k_multi(
         ctx.handle, n, ptrs, _lib.ptr(frames), C, rate, fmt, _lib.ptr(out), _lib.ptr(off), _lib._c.c_void_p(st.cuda_stream)),
         'iss_resample_to16k_multi')
+
+
+def window_multi(ctx, pcms, win, rate, out, stream=None):
+    """Windows of streams of one rate, channel count and dtype in one launch (iss_resample_window_multi): pcms[i] is a
+    contiguous CUDA tensor holding frames [f_base, n_known) of stream i, win an int64 array of rows (f_base, n_known,
+    k_first, n_out, out_off, flags); the outputs go to the int16 CUDA tensor `out`."""
+    x0 = pcms[0]
+    fmt = {torch.int16: _lib.PCM_S16, torch.float32: _lib.PCM_F32}[x0.dtype]
+    C = channels(x0)
+    assert all(p.is_cuda and p.is_contiguous() and p.dtype == x0.dtype and channels(p) == C for p in pcms)
+    _ensure_taps(ctx, rate)
+    n = len(pcms)
+    ptrs = (_lib._c.c_void_p * n)(*[p.data_ptr() for p in pcms])
+    win = np.ascontiguousarray(win, dtype=np.int64).reshape(n, 6)
+    st = stream if stream is not None else torch.cuda.current_stream(x0.device)
+    _lib.check(_lib.load().iss_resample_window_multi(
+        ctx.handle, n, ptrs, _lib.ptr(win), C, rate, fmt, _lib.ptr(out), _lib._c.c_void_p(st.cuda_stream)),
+        'iss_resample_window_multi')
 
 
 def resample_pass(ctx, pcms, rates):

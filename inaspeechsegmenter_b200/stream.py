@@ -14,6 +14,11 @@ Pipeline of one call (``_run``), every stage over all streams at once:
 Each chain is continued from its carried scores and emits the states that are final (``iss_viterbi_online``): the
 states up to the latest step where the backtracks from all K current states meet, or all of them when the chain ends.
 
+Streams at another rate or channel count (any integer rate from 8 to 192 kHz, 1 to 8 channels) are first resampled
+to 16 kHz mono int16 chunk by chunk (``resample.ready_outputs`` / ``end_outputs`` / ``first_kept``, DESIGN.md "Resampled
+streams"): the 16 kHz samples a stream's calls produce concatenate to ``resample.to16k`` on the whole stream, and the
+pipeline above runs on them as on a 16 kHz int16 stream.
+
 The device work sits behind a backend object (``CudaBackend``) so that the same orchestration can run against a CPU
 oracle in the tests.  The host keeps only small per-stream counters and the decided label tracks not yet returned.
 """
@@ -22,7 +27,7 @@ import warnings
 import numpy as np
 import torch
 
-from . import _lib, engine, pack
+from . import _lib, engine, pack, resample
 
 PATCH_W, LFILL = pack.PATCH_W, pack.PATCH_LFILL
 _UNDECIDED, _PASS = -1, -2         # per-patch output of a stage: not yet known / patch not in the stage's input label
@@ -82,8 +87,10 @@ class _Stage:
 
 class _Stream:
     def __init__(self, key, sid, kind):
-        self.key, self.sid, self.kind = key, sid, kind
-        self.samples = 0               # samples fed
+        self.key, self.sid, self.kind = key, sid, kind        # kind: (where, dtype, rate, channels)
+        self.rate = kind[2] if kind[2:] != (resample.TARGET_RATE, 1) else None    # resampled streams: their rate
+        self.frames_in = 0             # frames fed at the stream's own rate (resampled streams)
+        self.samples = 0               # 16 kHz samples fed
         self.F = 0                     # frames computed
         self.R0 = 0                    # first frame still retained on the device
         self.calibrated = False
@@ -98,22 +105,33 @@ class _Stream:
 
 
 def _kind(chunk, rate):
-    """(where, dtype name) of a chunk, or the error a chunk of another sort raises."""
-    if rate != 16000:
-        raise ValueError('live streams take 16 kHz audio, got sample_rate=%r' % (rate,))
-    if isinstance(chunk, torch.Tensor):
-        if chunk.dim() != 1:
-            raise ValueError('a stream chunk is 1-D (16 kHz mono), got shape %s' % (tuple(chunk.shape),))
-        if chunk.dtype not in (torch.int16, torch.float32):
+    """(kind, chunk): the (where, dtype name, rate, channels) of a chunk, and the chunk as the pipeline takes it: 16 kHz
+    mono ([frames] or [frames, 1]) 1-D, any other as resample.as_input returns it.  Raises the error a chunk of another
+    sort raises."""
+    rate = resample.check_rate(rate)
+    if not isinstance(chunk, (torch.Tensor, np.ndarray)):
+        raise TypeError('a stream chunk is a numpy array or a torch tensor, got %s' % type(chunk).__name__)
+    where = 'cuda' if isinstance(chunk, torch.Tensor) and chunk.is_cuda else 'host'
+    if resample.is_native(chunk, rate):
+        name = str(chunk.dtype).replace('torch.', '')
+        if name not in ('int16', 'float32'):
             raise TypeError('stream chunks are int16 or float32, got %s' % chunk.dtype)
-        return ('cuda' if chunk.is_cuda else 'host', str(chunk.dtype).replace('torch.', ''))
-    if isinstance(chunk, np.ndarray):
-        if chunk.ndim != 1:
-            raise ValueError('a stream chunk is 1-D (16 kHz mono), got shape %s' % (chunk.shape,))
-        if chunk.dtype not in (np.int16, np.float32):
-            raise TypeError('stream chunks are int16 or float32, got %s' % chunk.dtype)
-        return ('host', chunk.dtype.name)
-    raise TypeError('a stream chunk is a numpy array or a torch tensor, got %s' % type(chunk).__name__)
+        return (where, name, rate, 1), chunk.reshape(-1)
+    x = resample.as_input(chunk)
+    return (where, str(x.dtype).replace('torch.', ''), rate, resample.channels(x)), x
+
+
+def _khz(rate):
+    return '%g kHz' % (rate / 1000)
+
+
+def _check_same(key, opened, got):
+    if opened[:2] != got[:2]:
+        raise TypeError('stream %r was opened with %s %s chunks, got %s %s' % ((key,) + opened[:2] + got[:2]))
+    if opened[2] != got[2]:
+        raise ValueError('stream %r was opened at %s, got %s' % (key, _khz(opened[2]), _khz(got[2])))
+    if opened[3] != got[3]:
+        raise ValueError('stream %r was opened with %d channels, got %d' % (key, opened[3], got[3]))
 
 
 class LiveStreams:
@@ -150,18 +168,42 @@ class LiveStreams:
 
     def feed(self, chunks, sample_rate=16000):
         """Feed one chunk per key (opening the streams not seen before); returns {key: segments decided now}.
-        Invalid chunks raise before anything changes.  If the device pass itself fails, the object cannot be used
-        again: every later call raises."""
+        ``sample_rate`` is the rate of every chunk, or a dict {key: rate}.  A chunk is int16 or float32, [frames] or
+        [frames, channels], a numpy array, a CPU tensor or a CUDA tensor; a stream's location, dtype, rate and channel
+        count are those of its first chunk.  Streams other than 16 kHz mono are resampled to 16 kHz mono int16 on
+        the device, chunk by chunk, as ``segment_signal(x, sample_rate=rate)`` resamples the whole stream.  Invalid
+        chunks raise before anything changes.  If the device pass itself fails, the object cannot be used again: every
+        later call raises."""
         self._usable()
-        kinds = {k: _kind(c, sample_rate) for k, c in chunks.items()}
-        for k, kind in kinds.items():
+        if isinstance(sample_rate, dict):
+            missing = [k for k in chunks if k not in sample_rate]
+            if missing:
+                raise ValueError('no sample rate for stream %r in the sample_rate dict' % (missing[0],))
+            checked = {k: _kind(c, sample_rate[k]) for k, c in chunks.items()}
+        else:
+            checked = {k: _kind(c, sample_rate) for k, c in chunks.items()}
+        for k, (kind, _) in checked.items():
             st = self.streams.get(k)
-            if st is not None and st.kind != kind:
-                raise TypeError('stream %r was opened with %s %s chunks, got %s %s' % ((k,) + st.kind + kind))
-        for k, kind in kinds.items():
+            if st is not None:
+                _check_same(k, st.kind, kind)
+        for k, (kind, _) in checked.items():
             if k not in self.streams:
                 self.streams[k] = _Stream(k, self._new_sid(), kind)
-        return self._guarded(self._run, {self.streams[k]: c for k, c in chunks.items()}, [])
+        return self._guarded(self._feed, {self.streams[k]: c for k, (_, c) in checked.items()})
+
+    def _feed(self, chunks):
+        rs = [st for st in chunks if st.rate is not None]
+        if rs:
+            got = self.backend.resample({st.sid: chunks[st] for st in rs}, {st.sid: st.rate for st in rs})
+            for st in rs:
+                st.frames_in += int(chunks[st].shape[0])
+                chunks[st] = got[st.sid]
+        return self._run(chunks, [])
+
+    @staticmethod
+    def _samples_at_end(st):
+        """16 kHz samples of a stream once it ends (a resampled stream's last outputs come with the end)."""
+        return st.samples if st.rate is None else resample.end_outputs(st.frames_in, st.rate)
 
     def end(self, keys):
         self._usable()
@@ -169,24 +211,35 @@ class LiveStreams:
         unknown = [k for k in keys if k not in self.streams]
         if unknown:
             raise KeyError('no open stream %r' % (unknown[0],))
-        short = [k for k in keys if self.streams[k].samples < pack.WIN]
+        # counted before the resampler's flush, from the count the flush brings a stream to, so that a rejected end
+        # leaves the other streams as they were
+        short = [k for k in keys if self._samples_at_end(self.streams[k]) < pack.WIN]
         if short:
             st = self._close(self.streams[short[0]])
-            raise ValueError('media <array> holds %d samples: less than one 25 ms analysis frame' % st.samples)
+            raise ValueError('media <array> holds %d samples: less than one 25 ms analysis frame'
+                             % self._samples_at_end(st))
         return self._guarded(self._end, [self.streams[k] for k in keys])
 
     def _end(self, ending):
-        out = {}
+        out = {st.key: [] for st in ending}
+        rs = [st for st in ending if st.rate is not None]
+        if rs:
+            # flush the resampler first: its last outputs (those that read the zeros past the end) are the stream's
+            # last 16 kHz samples, and may complete its calibration
+            last = self.backend.resample({}, {st.sid: st.rate for st in rs}, [st.sid for st in rs])
+            for k, v in self._run({st: last[st.sid] for st in rs}, []).items():
+                out[k] += v
         offline = [st for st in ending if not st.calibrated]
         for st in offline:
             with warnings.catch_warnings():
                 warnings.simplefilter('ignore')
-                out[st.key] = self.backend.offline(st.sid, st.F)
+                out[st.key] += self.backend.offline(st.sid, st.F)
         live = [st for st in ending if st.calibrated]
         for st in live:
             st.ended = True
         if live:
-            out.update(self._run({}, live))
+            for k, v in self._run({}, live).items():
+                out[k] += v
         for st in ending:
             self._close(st)
         return {st.key: out[st.key] for st in ending}
@@ -370,6 +423,7 @@ class CudaBackend:
                           torch.zeros((0, 256), dtype=torch.uint8, device=self.dev)] for n in ('vad', 'gender')}
         self.free = {'vad': [], 'gender': []}
         self.nslot = {'vad': 0, 'gender': 0}
+        self.rs = {}                   # sid -> _RsTail of a resampled stream
 
     # slots of CNN chains
     def new_slot(self, name):
@@ -382,6 +436,7 @@ class CudaBackend:
         self.free[name].append(slot)
 
     def release(self, sid):
+        self.rs.pop(sid, None)
         self.tails.pop(sid, None)
         self.rows.pop(sid, None)
         self.frames.pop(sid, None)
@@ -402,6 +457,51 @@ class CudaBackend:
         s2[:scores.shape[0]] = scores
         h2[:hist.shape[0], :hist.shape[1]] = hist
         return s2, h2
+
+    def resample(self, chunks, rates, final=()):
+        """{sid: the 16 kHz int16 samples that become final}: chunks {sid: the stream's next frames, as _kind returns
+        them} at rates[sid], and for the streams in `final` (which have ended) all their remaining samples.  Each
+        stream keeps its raw input from resample.first_kept on; its tail and new chunk are one window.  Host chunks go
+        up in one pinned copy; each (rate, channels, dtype) group is one concatenation and one launch, into one int16
+        buffer whose views are returned."""
+        sids = sorted(set(chunks) | set(final))
+        fed = [s for s in sids if s in chunks]
+        staged = dict(zip(fed, self._stage_pass([chunks[s] for s in fed], self.dev))) if fed else {}
+        groups, n_out, pos = {}, {}, 0
+        for sid in sids:
+            t = self.rs.get(sid)
+            if t is None:
+                c = staged[sid]
+                t = self.rs[sid] = _RsTail(rates[sid], resample.channels(c), c.dtype)
+            n = t.n + (int(staged[sid].shape[0]) if sid in staged else 0)
+            k_to = (resample.end_outputs if sid in final else resample.ready_outputs)(n, t.rate)
+            n_out[sid] = (pos, k_to - t.k)
+            pos += k_to - t.k
+            groups.setdefault((t.rate, t.C, t.dtype), []).append((sid, n, k_to))
+        out = torch.empty(pos, dtype=torch.int16, device=self.dev)
+        for (rate, C, _), items in groups.items():
+            pieces = []
+            for sid, _, _ in items:
+                t = self.rs[sid]
+                pieces += [p for p in (t.tail, staged[sid].reshape(-1) if sid in staged else None) if p is not None]
+            big = torch.cat(pieces)
+            wins, rows, tails, at = [], [], [], 0
+            for sid, n, k_to in items:
+                t = self.rs[sid]
+                win = big[at:at + (n - t.f0) * C]
+                at += win.numel()
+                wins.append(win.view(-1, C))
+                rows.append((t.f0, n, t.k, k_to - t.k, n_out[sid][0], _lib.RESAMPLE_END if sid in final else 0))
+                keep = min(resample.first_kept(k_to, rate), n)
+                tails.append(win[(keep - t.f0) * C:])
+                t.f0, t.n, t.k = keep, n, k_to
+            resample.window_multi(self.ctx, wins, np.array(rows, dtype=np.int64), rate, out)
+            # the tails (a few ms each) get a buffer of their own, so that `big` is freed after this call
+            tb, at = torch.cat(tails), 0
+            for (sid, _, _), tl in zip(items, tails):
+                self.rs[sid].tail = tb[at:at + tl.numel()]
+                at += tl.numel()
+        return {sid: out[a:a + k] for sid, (a, k) in n_out.items()}
 
     def ingest(self, chunks, keep):
         """Append each chunk to its stream, compute the new frames (K1 on tail + chunk) and rebuild the store with the
@@ -556,6 +656,15 @@ class CudaBackend:
             difflen = W - F
             mspec = torch.cat((mspec, mspec.min().expand(difflen, 24)))
         return self.seg.segment_feats(mspec.contiguous(), loge.contiguous(), difflen, 0)
+
+
+class _RsTail:
+    """The resampler state of a stream: its raw samples of frames [f0, n) (flattened) and its next output k."""
+    __slots__ = ('rate', 'C', 'dtype', 'tail', 'f0', 'n', 'k')
+
+    def __init__(self, rate, C, dtype):
+        self.rate, self.C, self.dtype = rate, C, dtype
+        self.tail, self.f0, self.n, self.k = None, 0, 0, 0
 
 
 class _Layout:

@@ -39,7 +39,7 @@ typedef struct iss_mlp iss_mlp;
 
 /* ---- library / context ------------------------------------------------- */
 
-#define ISS_ABI_VERSION 6
+#define ISS_ABI_VERSION 7
 int         iss_version(void);               /* == ISS_ABI_VERSION of the header the library was built from */
 const char *iss_last_error(void);
 /* Creates a context bound to CUDA device `device` (one per host thread that
@@ -330,6 +330,21 @@ int iss_resample_release_taps(iss_ctx *ctx, int rate);
 int iss_resample_to16k_multi(iss_ctx *ctx, int n_rec, const void *const *h_pcm, const int64_t *h_n_frames,
                              int channels, int rate, int pcm_format, int16_t *d_out, const int64_t *h_out_off,
                              void *stream);
+/* The same resampling over windows of streams fed piece by piece (live streams), n_rec
+ * records of one (rate, channels, pcm_format) in one launch.  Record r is the int64 row
+ * h_win[6 r ..] = {f_base, n_known, k_first, n_out, out_off, flags}: h_pcm[r] (a DEVICE
+ * pointer) holds frames [f_base, n_known) of its stream, and outputs k_first ..
+ * k_first + n_out - 1 of the stream go to d_out[out_off ..].  Frames at or past n_known
+ * read as zero, which is the definition's padding only once the stream has ended
+ * (flags ISS_RESAMPLE_END).  Every output equals, bit for bit, the same output of
+ * iss_resample_to16k_multi on the whole stream.  Output k reads frames a + s_q ..
+ * a + s_q + n_q - 1 (k down = a up + q, the phase table of iss_resample_upload_taps).
+ * Checked on the host before the launch, ISS_ERR_INVALID with the record's index: no
+ * output reads a frame in [0, f_base); without ISS_RESAMPLE_END no output reads a frame at
+ * or past n_known; k_first + n_out <= iss_resample_num_frames(n_known, rate). */
+#define ISS_RESAMPLE_END 1
+int iss_resample_window_multi(iss_ctx *ctx, int n_rec, const void *const *h_pcm, const int64_t *h_win,
+                              int channels, int rate, int pcm_format, int16_t *d_out, void *stream);
 
 /* ---- K5: ResNet101 x-vector extractor ----------------------------------------
  * Replaces VBxExtractor.get_embedding / OnnxBackendExtractor (vbx_segmenter.py:
