@@ -8,16 +8,25 @@
 // Exactness: the forward recursion is evaluated in IEEE double in exactly the
 // reference's order of operations (so every argmax decision sees the same bits);
 // that chain is inherently serial, so the forward pass runs one warp per
-// sequence: the 32 lanes fetch and convert 32 steps of emissions in parallel
+// chain: the 32 lanes fetch and convert 32 steps of emissions in parallel
 // (coalesced), then replay them through register shuffles while every lane
 // carries the same V; lane j keeps step j's back-pointer byte so stores are
-// coalesced too.  The backtrack -- pure integer function composition, hence
-// associative and exact -- is parallel: per-256-step chunk maps, a short serial
-// scan over chunk maps, then all chunks emit their states concurrently.
+// coalesced too (forward_steps).  The backtrack -- pure integer function
+// composition, hence associative and exact -- is parallel: per-256-step chunk
+// maps, a short serial scan over chunk maps, then all chunks emit their states
+// concurrently.
+//
+// Structure: an offline entry point carves its workspace with carve(), whose
+// layout depends only on the sizes of the decode, names the chains of each
+// forward launch with a VitChains (which sequence a block walks, where its
+// scores come from and go to, where its argmax and back-pointers go), and
+// backtracks with run_backtrack.  The online kernel for live streams runs the
+// same forward_steps and traces back its own history rows.
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
 #include <algorithm>
+#include <type_traits>
 #include <vector>
 
 #include "iss_common.cuh"
@@ -26,6 +35,7 @@ namespace {
 
 constexpr int CH = 256;            // backtrack chunk (steps)
 constexpr int MAXK = 4;
+constexpr int64_t ECH = 16384;     // chunk of the chunk-parallel energy decode (steps)
 
 struct VitParams {
     double A[MAXK][MAXK];          // from -> to
@@ -34,21 +44,78 @@ struct VitParams {
     double log_ratio;
 };
 
-struct VitLayout {
+// energy mode (K = 2) when h_emis is given, CNN posteriors otherwise
+VitParams make_params(int K, const double *h_trans, double log_prior, const double *h_emis, double log_ratio)
+{
+    VitParams prm = {};
+    for (int i = 0; i < K; ++i) for (int j = 0; j < K; ++j) prm.A[i][j] = h_trans[i * K + j];
+    prm.prior = log_prior;
+    if (h_emis) { prm.emis_hit = h_emis[0]; prm.emis_miss = h_emis[1]; prm.log_ratio = log_ratio; }
+    return prm;
+}
+
+size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+
+// The regions of d_work.  A chain is one warp's forward walk over one sequence, or over one ECH chunk of it.
+struct VitWork {
     uint8_t *bp;                   // [total] one byte per step: 2 bits per destination state
-    uint8_t *cmap;                 // [nchunks] composite map per chunk
-    uint8_t *cend;                 // [nchunks] state at the last step of each chunk
-    int64_t *seg_off;              // [n_seg+1]
-    int64_t *chunk_off;            // [n_seg+1]
-    uint8_t *last;                 // [n_seg] argmax V[T-1]
-    // partial-chain support (time-sharded recordings)
-    const double *vin;             // [n_seg][MAXK] incoming scores (continue from a predecessor) or nullptr
-    double *vout;                  // [n_seg][MAXK] outgoing scores V[T-1] or nullptr
-    int alias;                     // 1: every block walks the SAME range seg_off[0..1] (basis chains of a transfer matrix)
-                                   // 2: block b walks segment b / 2 with vin / vout slot b (two basis chains per segment)
-    int store_bp;                  // 0: scores only
-    int stats_stride;              // energy mode: sequence s thresholds on stats[s * stats_stride ..] (0: one shared pair)
-    const int64_t *out_off;        // [n_seg] first output of each sequence when out_stride > 1, or nullptr (single sequence)
+    uint8_t *cmap;                 // [chunks] composite back map of each backtrack chunk
+    uint8_t *cend;                 // [chunks] state at the last step of each backtrack chunk
+    int64_t *seq_off;              // [n_seq + 1] steps of each sequence
+    int64_t *chunk_off;            // [n_seq + 1] backtrack chunks of each sequence
+    int64_t *out_off;              // [n_seq] first output of each sequence (several recordings)
+    uint8_t *last;                 // [chains] first argmax of each chain's final scores
+    double *vin;                   // [chains][MAXK] incoming scores of each chain
+    double *vout;                  // [chains][MAXK] outgoing scores V[T-1] of each chain
+    uint8_t *map;                  // [1] composite back map of the whole of sequence 0
+    int64_t *ech_off;              // [n_ech + 1] chunk-parallel energy decode: steps of each ECH chunk
+    double *entry;                 // [n_ech][MAXK] scores entering each ECH chunk
+    size_t bytes;
+};
+
+// The one layout of d_work for a decode of `total` steps in n_seq sequences, a function of the sizes only: so
+// iss_energy_forward and iss_energy_emit find the same tables in the d_work they share, and iss_viterbi_work_bytes
+// is the layout on a null base.
+VitWork carve(void *base, int64_t total, int n_seq)
+{
+    const int64_t chunks = total / CH + n_seq;                          // >= the chunks of any n_seq sequences
+    const int64_t n_ech = (total + ECH - 1) / ECH;
+    const int64_t chains = std::max<int64_t>(n_seq, 2 * n_ech);         // one per sequence or two per ECH chunk
+    VitWork w;
+    size_t o = 0;
+    auto take = [&](auto *&p, int64_t n) {
+        p = reinterpret_cast<std::remove_reference_t<decltype(p)>>(reinterpret_cast<uintptr_t>(base) + o);
+        o = align_up(o + sizeof(*p) * (size_t)n, 256);
+    };
+    take(w.bp, total);
+    take(w.cmap, chunks);
+    take(w.cend, chunks);
+    take(w.seq_off, n_seq + 1);
+    take(w.chunk_off, n_seq + 1);
+    take(w.out_off, n_seq);
+    take(w.last, chains);
+    take(w.vin, chains * MAXK);
+    take(w.vout, chains * MAXK);
+    take(w.map, 1);
+    take(w.ech_off, n_ech + 1);
+    take(w.entry, n_ech * MAXK);
+    w.bytes = o;
+    return w;
+}
+
+// The chains of one forward launch: block b walks sequence s = first + b / per_seq of seq_off as chain
+// c = first * per_seq + b (per_seq = 2: the two basis chains of a transfer matrix).  Chain c starts from the scores
+// vin[c], or from the prior on the sequence's first step when vin is null; it leaves its final scores in vout[c] and
+// their first argmax in last[c], and its back-pointers at the sequence's steps of bp, where those are not null.
+// Energy mode thresholds sequence s on stats[s * stats_stride ..].
+struct VitChains {
+    const int64_t *seq_off;
+    int first, per_seq;
+    const double *vin;
+    double *vout;
+    uint8_t *last;
+    uint8_t *bp;
+    int stats_stride;
 };
 
 __device__ __forceinline__ bool better(double c, double best)
@@ -140,31 +207,23 @@ __device__ __forceinline__ unsigned compose_map(unsigned f, unsigned m)
     return r;
 }
 
-template <int K, bool ENERGY>
-__global__ void __launch_bounds__(32)
-viterbi_forward_kernel(const float *__restrict__ src, const double *__restrict__ stats, VitParams prm, VitLayout lay)
+// Steps [0, T) of one chain whose emissions start at step s0 of src, with every lane carrying the same V.  `first`:
+// step 0 is the first step of the sequence (the prior).  Lane i of each round of 32 steps hands the back-pointer
+// byte of step t = base + i to store(t, byte).
+template <int K, bool ENERGY, typename Store>
+__device__ __forceinline__ void forward_steps(const float *__restrict__ src, int64_t s0, int64_t T, double thr,
+                                              const VitParams &prm, bool first, double (&V)[K], Store store)
 {
-    const int slot = blockIdx.x, lane = threadIdx.x;             // slot indexes vin / vout / last
-    const int seg = lay.alias == 1 ? 0 : (lay.alias == 2 ? slot >> 1 : slot);
-    const int64_t t0 = lay.seg_off[seg];
-    const int64_t T = lay.seg_off[seg + 1] - t0;
-    if (T <= 0) return;
-    const bool cont = lay.vin != nullptr;          // first step is an ordinary transition from vin
-    const double thr = ENERGY ? energy_threshold(stats + (int64_t)seg * lay.stats_stride, prm.log_ratio) : 0.0;
-    double V[K];
-#pragma unroll
-    for (int j = 0; j < K; ++j) V[j] = cont ? lay.vin[slot * MAXK + j] : 0.0;
-
+    const int lane = threadIdx.x;
     for (int64_t base = 0; base < T; base += 32) {
         const int64_t t = base + lane;
         double e[K];
 #pragma unroll
         for (int j = 0; j < K; ++j) e[j] = 0.0;
-        if (t < T) load_emissions<K, ENERGY>(src, t0 + t, thr, prm, e);
+        if (t < T) load_emissions<K, ENERGY>(src, s0 + t, thr, prm, e);
         const int nstep = (int)min((int64_t)32, T - base);
         unsigned mybp = 0;
-        auto dp_step = [&](const double (&es)[K], bool is_first) -> unsigned { return vit_step<K, ENERGY>(V, es, prm, is_first); };
-        if (nstep == 32 && (base > 0 || cont)) {
+        if (nstep == 32 && (base > 0 || !first)) {
             // full block, fully unrolled: the 32 x K emission shuffles do not depend on V, so they are
             // issued ahead and only the add/compare/select chain remains on the serial critical path
 #pragma unroll
@@ -172,7 +231,7 @@ viterbi_forward_kernel(const float *__restrict__ src, const double *__restrict__
                 double es[K];
 #pragma unroll
                 for (int j = 0; j < K; ++j) es[j] = __shfl_sync(0xffffffffu, e[j], s);
-                const unsigned bp = dp_step(es, false);
+                const unsigned bp = vit_step<K, ENERGY>(V, es, prm, false);
                 mybp = (lane == s) ? bp : mybp;
             }
         } else {
@@ -180,25 +239,42 @@ viterbi_forward_kernel(const float *__restrict__ src, const double *__restrict__
                 double es[K];
 #pragma unroll
                 for (int j = 0; j < K; ++j) es[j] = __shfl_sync(0xffffffffu, e[j], s);
-                const unsigned bp = dp_step(es, base + s == 0 && !cont);
+                const unsigned bp = vit_step<K, ENERGY>(V, es, prm, first && base + s == 0);
                 if (lane == s) mybp = bp;
             }
         }
-        if (t < T && lay.store_bp) lay.bp[t0 + t] = (uint8_t)mybp;
+        if (t < T) store(t, mybp);
     }
-    if (lane == 0) {
-        const int arg = first_argmax<K>(V);
-        if (lay.store_bp) lay.last[slot] = (uint8_t)arg;
-        if (lay.vout) {
+}
+
+template <int K, bool ENERGY>
+__global__ void __launch_bounds__(32)
+viterbi_forward_kernel(const float *__restrict__ src, const double *__restrict__ stats, VitParams prm, VitChains ch)
+{
+    const int c = ch.first * ch.per_seq + blockIdx.x, s = c / ch.per_seq;
+    const int64_t t0 = ch.seq_off[s];
+    const int64_t T = ch.seq_off[s + 1] - t0;
+    if (T <= 0) return;
+    const bool cont = ch.vin != nullptr;           // first step is an ordinary transition from vin
+    const double thr = ENERGY ? energy_threshold(stats + (int64_t)s * ch.stats_stride, prm.log_ratio) : 0.0;
+    double V[K];
 #pragma unroll
-            for (int k = 0; k < K; ++k) lay.vout[slot * MAXK + k] = V[k];
+    for (int j = 0; j < K; ++j) V[j] = cont ? ch.vin[c * MAXK + j] : 0.0;
+    forward_steps<K, ENERGY>(src, t0, T, thr, prm, !cont, V, [&](int64_t t, unsigned b) {
+        if (ch.bp) ch.bp[t0 + t] = (uint8_t)b;
+    });
+    if (threadIdx.x == 0) {
+        if (ch.last) ch.last[c] = (uint8_t)first_argmax<K>(V);
+        if (ch.vout) {
+#pragma unroll
+            for (int k = 0; k < K; ++k) ch.vout[c * MAXK + k] = V[k];
         }
     }
 }
 
-__device__ __forceinline__ int find_seg(const int64_t *chunk_off, int n_seg, int64_t c)
+__device__ __forceinline__ int find_seg(const int64_t *chunk_off, int n_seq, int64_t c)
 {
-    int lo = 0, hi = n_seg;            // chunk_off[lo] <= c < chunk_off[hi]
+    int lo = 0, hi = n_seq;            // chunk_off[lo] <= c < chunk_off[hi]
     while (hi - lo > 1) {
         const int mid = (lo + hi) >> 1;
         if (chunk_off[mid] <= c) lo = mid; else hi = mid;
@@ -207,53 +283,52 @@ __device__ __forceinline__ int find_seg(const int64_t *chunk_off, int n_seg, int
 }
 
 // cmap[c]: (state at the last step of chunk c) -> (state at the last step of chunk c-1)
-__global__ void viterbi_chunk_map_kernel(VitLayout lay, int n_seg, int64_t nchunks, int has_pred)
+__global__ void viterbi_chunk_map_kernel(VitWork w, int n_seq, int64_t nchunks, int has_pred)
 {
     const int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= nchunks) return;
-    const int seg = find_seg(lay.chunk_off, n_seg, c);
-    const int64_t t0 = lay.seg_off[seg], T = lay.seg_off[seg + 1] - t0;
-    const int64_t lc = c - lay.chunk_off[seg];
+    const int seg = find_seg(w.chunk_off, n_seq, c);
+    const int64_t t0 = w.seq_off[seg], T = w.seq_off[seg + 1] - t0;
+    const int64_t lc = c - w.chunk_off[seg];
     const int64_t a = lc * CH, b = min(a + CH, T);          // steps [a, b)
     unsigned m = 0xE4;                                      // identity: 3,2,1,0 in 2-bit fields
-    const uint8_t *bp = lay.bp + t0;
+    const uint8_t *bp = w.bp + t0;
     for (int64_t t = b - 1; t >= a; --t) {
         if (t == 0 && !has_pred) break;                     // bp[0] is unused when the sequence has no predecessor
-        const unsigned f = bp[t];
-        unsigned r = 0;
-#pragma unroll
-        for (int x = 0; x < 4; ++x) r |= ((f >> (2 * ((m >> (2 * x)) & 3))) & 3) << (2 * x);
-        m = r;
+        m = compose_map(bp[t], m);
     }
-    lay.cmap[c] = (uint8_t)m;
+    w.cmap[c] = (uint8_t)m;
 }
 
-// serial over the chunks of one segment (T/256 steps), one thread per segment
-__global__ void viterbi_chunk_scan_kernel(VitLayout lay, int n_seg)
+// serial over the chunks of one sequence (T/256 steps), one thread per sequence, which starts from the argmax of
+// chain end_chain + seg (the chain that walked its last step)
+__global__ void viterbi_chunk_scan_kernel(VitWork w, int n_seq, int end_chain)
 {
     const int seg = blockIdx.x * blockDim.x + threadIdx.x;
-    if (seg >= n_seg) return;
-    const int64_t c0 = lay.chunk_off[seg], c1 = lay.chunk_off[seg + 1];
+    if (seg >= n_seq) return;
+    const int64_t c0 = w.chunk_off[seg], c1 = w.chunk_off[seg + 1];
     if (c1 <= c0) return;
-    unsigned x = lay.last[seg];
+    unsigned x = w.last[end_chain + seg];
     for (int64_t c = c1 - 1; c >= c0; --c) {
-        lay.cend[c] = (uint8_t)x;
-        x = (lay.cmap[c] >> (2 * x)) & 3;
+        w.cend[c] = (uint8_t)x;
+        x = (w.cmap[c] >> (2 * x)) & 3;
     }
 }
 
-__global__ void viterbi_chunk_emit_kernel(VitLayout lay, int n_seg, int64_t nchunks, int out_stride,
-                                          uint8_t *__restrict__ states)
+// every out_stride-th state of sequence seg to states[out_off[seg] ..], or to states[seq_off[seg] ..] when out_off is
+// null (a single sequence has seq_off[0] == 0)
+__global__ void viterbi_chunk_emit_kernel(VitWork w, int n_seq, int64_t nchunks, const int64_t *__restrict__ out_off,
+                                          int out_stride, uint8_t *__restrict__ states)
 {
     const int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= nchunks) return;
-    const int seg = find_seg(lay.chunk_off, n_seg, c);
-    const int64_t t0 = lay.seg_off[seg], T = lay.seg_off[seg + 1] - t0;
-    const int64_t lc = c - lay.chunk_off[seg];
+    const int seg = find_seg(w.chunk_off, n_seq, c);
+    const int64_t t0 = w.seq_off[seg], T = w.seq_off[seg + 1] - t0;
+    const int64_t lc = c - w.chunk_off[seg];
     const int64_t a = lc * CH, b = min(a + CH, T);
-    const uint8_t *bp = lay.bp + t0;
-    unsigned x = lay.cend[c];
-    const int64_t o0 = lay.out_off ? lay.out_off[seg] : t0;         // a single sequence has t0 == 0
+    const uint8_t *bp = w.bp + t0;
+    unsigned x = w.cend[c];
+    const int64_t o0 = out_off ? out_off[seg] : t0;
     for (int64_t t = b - 1; t >= a; --t) {
         if (out_stride == 1) states[o0 + t] = (uint8_t)x;
         else if (t % out_stride == 0) states[o0 + t / out_stride] = (uint8_t)x;
@@ -261,170 +336,64 @@ __global__ void viterbi_chunk_emit_kernel(VitLayout lay, int n_seg, int64_t nchu
     }
 }
 
-size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
-
-struct HostPlan {
-    std::vector<int64_t> seg_off, chunk_off;
-    int64_t total, nchunks;
-};
-
-int make_layout(const int64_t *h_seg_off, int n_seg, void *d_work, HostPlan &hp, VitLayout &lay, cudaStream_t st)
-{
-    hp.seg_off.assign(h_seg_off, h_seg_off + n_seg + 1);
-    hp.chunk_off.resize(n_seg + 1);
-    int64_t nc = 0;
-    for (int s = 0; s < n_seg; ++s) {
-        hp.chunk_off[s] = nc;
-        const int64_t T = h_seg_off[s + 1] - h_seg_off[s];
-        ISS_REQUIRE(T >= 0, ISS_ERR_INVALID, "viterbi: segment offsets must be non-decreasing");
-        nc += (T + CH - 1) / CH;
-    }
-    hp.chunk_off[n_seg] = nc;
-    hp.total = h_seg_off[n_seg];
-    hp.nchunks = nc;
-    uint8_t *p = reinterpret_cast<uint8_t *>(d_work);
-    size_t o = 0;
-    lay.bp = p + o;        o = align_up(o + (size_t)hp.total, 256);
-    lay.cmap = p + o;      o = align_up(o + (size_t)nc, 256);
-    lay.cend = p + o;      o = align_up(o + (size_t)nc, 256);
-    lay.seg_off = reinterpret_cast<int64_t *>(p + o);   o = align_up(o + sizeof(int64_t) * (n_seg + 1), 256);
-    lay.chunk_off = reinterpret_cast<int64_t *>(p + o); o = align_up(o + sizeof(int64_t) * (n_seg + 1), 256);
-    lay.last = p + o;
-    ISS_CUDA_OK(cudaMemcpyAsync(lay.seg_off, hp.seg_off.data(), sizeof(int64_t) * (n_seg + 1), cudaMemcpyHostToDevice, st));
-    ISS_CUDA_OK(cudaMemcpyAsync(lay.chunk_off, hp.chunk_off.data(), sizeof(int64_t) * (n_seg + 1), cudaMemcpyHostToDevice, st));
-    return ISS_OK;
-}
-
-int run_backtrack(const VitLayout &lay, const HostPlan &hp, int n_seg, int out_stride, uint8_t *d_states, cudaStream_t st)
-{
-    if (hp.nchunks == 0) return ISS_OK;
-    const int TB = 128;
-    const unsigned gc = (unsigned)((hp.nchunks + TB - 1) / TB);
-    viterbi_chunk_map_kernel<<<gc, TB, 0, st>>>(lay, n_seg, hp.nchunks, 0);
-    viterbi_chunk_scan_kernel<<<(n_seg + 63) / 64, 64, 0, st>>>(lay, n_seg);
-    viterbi_chunk_emit_kernel<<<gc, TB, 0, st>>>(lay, n_seg, hp.nchunks, out_stride, d_states);
-    ISS_CUDA_OK(cudaGetLastError());
-    iss_count_launch(3);
-    return ISS_OK;
-}
-
 // composite of all chunk maps of sequence 0: (state at the last step) -> (state just before the first step)
-__global__ void viterbi_compose_kernel(VitLayout lay, int64_t nchunks, uint8_t *out)
+__global__ void viterbi_compose_kernel(VitWork w, int64_t nchunks)
 {
     if (threadIdx.x != 0 || blockIdx.x != 0) return;
     unsigned m = 0xE4;
-    for (int64_t c = nchunks - 1; c >= 0; --c) {
-        const unsigned f = lay.cmap[c];
-        unsigned r = 0;
-#pragma unroll
-        for (int x = 0; x < 4; ++x) r |= ((f >> (2 * ((m >> (2 * x)) & 3))) & 3) << (2 * x);
-        m = r;
+    for (int64_t c = nchunks - 1; c >= 0; --c) m = compose_map(w.cmap[c], m);
+    w.map[0] = (uint8_t)m;
+}
+
+// Uploads the offsets of n_seq sequences and of their backtrack chunks; *nchunks = the number of chunks.
+int upload_offsets(const VitWork &w, const int64_t *h_seq_off, int n_seq, int64_t *nchunks, cudaStream_t st)
+{
+    std::vector<int64_t> seq_off(h_seq_off, h_seq_off + n_seq + 1), chunk_off(n_seq + 1);
+    int64_t nc = 0;
+    for (int s = 0; s < n_seq; ++s) {
+        chunk_off[s] = nc;
+        const int64_t T = seq_off[s + 1] - seq_off[s];
+        ISS_REQUIRE(T >= 0, ISS_ERR_INVALID, "viterbi: segment offsets must be non-decreasing");
+        nc += (T + CH - 1) / CH;
     }
-    out[0] = (uint8_t)m;
+    chunk_off[n_seq] = nc;
+    *nchunks = nc;
+    ISS_CUDA_OK(cudaMemcpyAsync(w.seq_off, seq_off.data(), sizeof(int64_t) * (n_seq + 1), cudaMemcpyHostToDevice, st));
+    ISS_CUDA_OK(cudaMemcpyAsync(w.chunk_off, chunk_off.data(), sizeof(int64_t) * (n_seq + 1), cudaMemcpyHostToDevice, st));
+    return ISS_OK;
 }
 
-__global__ void viterbi_set_last_kernel(VitLayout lay, int state) { if (threadIdx.x == 0 && blockIdx.x == 0) lay.last[0] = (uint8_t)state; }
-
-}  // namespace
-
-// ---- partial chains of the energy Viterbi for time-sharded recordings (SURVEY 8(e)) -------------------
-static void fill_energy_params(VitParams &prm, const double *h_emis, const double *h_trans, double log_prior, double log_ratio)
+int run_backtrack(const VitWork &w, int n_seq, int64_t nchunks, int end_chain, const int64_t *out_off, int out_stride,
+                  uint8_t *d_states, cudaStream_t st)
 {
-    for (int i = 0; i < 2; ++i) for (int j = 0; j < 2; ++j) prm.A[i][j] = h_trans[i * 2 + j];
-    prm.prior = log_prior; prm.emis_hit = h_emis[0]; prm.emis_miss = h_emis[1]; prm.log_ratio = log_ratio;
+    if (nchunks == 0) return ISS_OK;
+    const int TB = 128;
+    const unsigned gc = (unsigned)((nchunks + TB - 1) / TB);
+    viterbi_chunk_map_kernel<<<gc, TB, 0, st>>>(w, n_seq, nchunks, 0);
+    viterbi_chunk_scan_kernel<<<(n_seq + 63) / 64, 64, 0, st>>>(w, n_seq, end_chain);
+    viterbi_chunk_emit_kernel<<<gc, TB, 0, st>>>(w, n_seq, nchunks, out_off, out_stride, d_states);
+    ISS_CUDA_OK(cudaGetLastError());
+    iss_count_launch(3);
+    return ISS_OK;
 }
 
-extern "C" int iss_energy_transfer(iss_ctx *ctx, const float *d_loge, int64_t L, const double *d_loge_stats,
-                                   double log_ratio, const double *h_emis, const double *h_trans,
-                                   double *h_matrix, void *d_work, void *stream)
+// One chain per sequence h_off[s] .. h_off[s+1] of src, then the backtrack: every out_stride-th state of sequence s
+// goes to d_states[h_out_off[s] ..], or to d_states[h_off[s] ..] when h_out_off is null.
+template <int K, bool ENERGY>
+int decode_sequences(const float *src, const int64_t *h_off, int n_seq, const double *stats, int stats_stride,
+                     const VitParams &prm, int out_stride, const int64_t *h_out_off, uint8_t *d_states, void *d_work,
+                     cudaStream_t st)
 {
-    ISS_REQUIRE(ctx && d_loge && d_loge_stats && h_emis && h_trans && h_matrix && d_work && L > 0, ISS_ERR_INVALID, "iss_energy_transfer: bad argument");
-    ISS_CUDA_OK(cudaSetDevice(ctx->device));
-    cudaStream_t st = iss_stream(stream);
-    const int64_t off[2] = {0, L};
-    HostPlan hp; VitLayout lay = {};
-    int rc = make_layout(off, 1, d_work, hp, lay, st);
+    const VitWork w = carve(d_work, h_off[n_seq], n_seq);
+    int64_t nc;
+    int rc = upload_offsets(w, h_off, n_seq, &nc, st);
     if (rc != ISS_OK) return rc;
-    // scratch for vin / vout lives behind `last`
-    double *d_v = reinterpret_cast<double *>(lay.last + 256);
-    const double NEG_INF = -INFINITY;
-    double vin[2 * MAXK] = {0.0, NEG_INF, 0, 0, NEG_INF, 0.0, 0, 0};      // basis vectors e_0, e_1 (max-plus)
-    ISS_CUDA_OK(cudaMemcpyAsync(d_v, vin, sizeof(vin), cudaMemcpyHostToDevice, st));
-    lay.vin = d_v; lay.vout = d_v + 2 * MAXK; lay.alias = 1; lay.store_bp = 0;
-    VitParams prm = {};
-    fill_energy_params(prm, h_emis, h_trans, 0.0, log_ratio);
-    viterbi_forward_kernel<2, true><<<2, 32, 0, st>>>(d_loge, d_loge_stats, prm, lay);
+    if (h_out_off) ISS_CUDA_OK(cudaMemcpyAsync(w.out_off, h_out_off, sizeof(int64_t) * n_seq, cudaMemcpyHostToDevice, st));
+    const VitChains ch = {w.seq_off, 0, 1, nullptr, nullptr, w.last, w.bp, stats_stride};
+    viterbi_forward_kernel<K, ENERGY><<<n_seq, 32, 0, st>>>(src, stats, prm, ch);
     ISS_CUDA_OK(cudaGetLastError());
     iss_count_launch();
-    double vout[2 * MAXK];
-    ISS_CUDA_OK(cudaMemcpyAsync(vout, lay.vout, sizeof(vout), cudaMemcpyDeviceToHost, st));
-    ISS_CUDA_OK(cudaStreamSynchronize(st));
-    // M[j][i] = score of ending in j having started (before the first frame) in i
-    for (int i = 0; i < 2; ++i) for (int j = 0; j < 2; ++j) h_matrix[j * 2 + i] = vout[i * MAXK + j];
-    return ISS_OK;
-}
-
-extern "C" int iss_energy_forward(iss_ctx *ctx, const float *d_loge, int64_t L, const double *d_loge_stats,
-                                  double log_ratio, const double *h_emis, const double *h_trans, double log_prior,
-                                  const double *h_vin, double *h_vout, uint8_t *h_backmap, void *d_work, void *stream)
-{
-    ISS_REQUIRE(ctx && d_loge && d_loge_stats && h_emis && h_trans && h_vout && h_backmap && d_work && L > 0, ISS_ERR_INVALID, "iss_energy_forward: bad argument");
-    ISS_CUDA_OK(cudaSetDevice(ctx->device));
-    cudaStream_t st = iss_stream(stream);
-    const int64_t off[2] = {0, L};
-    HostPlan hp; VitLayout lay = {};
-    int rc = make_layout(off, 1, d_work, hp, lay, st);
-    if (rc != ISS_OK) return rc;
-    double *d_v = reinterpret_cast<double *>(lay.last + 256);
-    if (h_vin) {
-        double vin[MAXK] = {h_vin[0], h_vin[1], 0, 0};
-        ISS_CUDA_OK(cudaMemcpyAsync(d_v, vin, sizeof(vin), cudaMemcpyHostToDevice, st));
-        lay.vin = d_v;
-    }
-    lay.vout = d_v + 2 * MAXK; lay.alias = 0; lay.store_bp = 1;
-    VitParams prm = {};
-    fill_energy_params(prm, h_emis, h_trans, log_prior, log_ratio);
-    viterbi_forward_kernel<2, true><<<1, 32, 0, st>>>(d_loge, d_loge_stats, prm, lay);
-    const unsigned gc = (unsigned)((hp.nchunks + 127) / 128);
-    viterbi_chunk_map_kernel<<<gc, 128, 0, st>>>(lay, 1, hp.nchunks, h_vin ? 1 : 0);
-    uint8_t *d_map = reinterpret_cast<uint8_t *>(d_v + 4 * MAXK);
-    viterbi_compose_kernel<<<1, 32, 0, st>>>(lay, hp.nchunks, d_map);
-    ISS_CUDA_OK(cudaGetLastError());
-    iss_count_launch(3);
-    double vout[MAXK];
-    uint8_t m;
-    ISS_CUDA_OK(cudaMemcpyAsync(vout, lay.vout, sizeof(vout), cudaMemcpyDeviceToHost, st));
-    ISS_CUDA_OK(cudaMemcpyAsync(&m, d_map, 1, cudaMemcpyDeviceToHost, st));
-    ISS_CUDA_OK(cudaStreamSynchronize(st));
-    h_vout[0] = vout[0]; h_vout[1] = vout[1];
-    h_backmap[0] = m & 3; h_backmap[1] = (m >> 2) & 3;
-    return ISS_OK;
-}
-
-extern "C" int iss_energy_emit(iss_ctx *ctx, int64_t L, int end_state, int out_stride, uint8_t *d_states,
-                               void *d_work, void *stream)
-{
-    ISS_REQUIRE(ctx && d_states && d_work && L > 0 && out_stride >= 1 && end_state >= -1 && end_state < 2, ISS_ERR_INVALID, "iss_energy_emit: bad argument");
-    ISS_CUDA_OK(cudaSetDevice(ctx->device));
-    cudaStream_t st = iss_stream(stream);
-    // same carve as iss_energy_forward (no copies: the tables are already on the device)
-    HostPlan hp; VitLayout lay = {};
-    hp.seg_off = {0, L}; hp.chunk_off = {0, (L + CH - 1) / CH}; hp.total = L; hp.nchunks = (L + CH - 1) / CH;
-    uint8_t *p = reinterpret_cast<uint8_t *>(d_work);
-    size_t o = 0;
-    lay.bp = p + o;        o = align_up(o + (size_t)hp.total, 256);
-    lay.cmap = p + o;      o = align_up(o + (size_t)hp.nchunks, 256);
-    lay.cend = p + o;      o = align_up(o + (size_t)hp.nchunks, 256);
-    lay.seg_off = reinterpret_cast<int64_t *>(p + o);   o = align_up(o + sizeof(int64_t) * 2, 256);
-    lay.chunk_off = reinterpret_cast<int64_t *>(p + o); o = align_up(o + sizeof(int64_t) * 2, 256);
-    lay.last = p + o;
-    if (end_state >= 0) viterbi_set_last_kernel<<<1, 32, 0, st>>>(lay, end_state);
-    const unsigned gc = (unsigned)((hp.nchunks + 127) / 128);
-    viterbi_chunk_scan_kernel<<<1, 64, 0, st>>>(lay, 1);
-    viterbi_chunk_emit_kernel<<<gc, 128, 0, st>>>(lay, 1, hp.nchunks, out_stride, d_states);
-    ISS_CUDA_OK(cudaGetLastError());
-    iss_count_launch(3);
-    return ISS_OK;
+    return run_backtrack(w, n_seq, nc, 0, h_out_off ? w.out_off : nullptr, out_stride, d_states, st);
 }
 
 // ---- chunk-parallel energy Viterbi ------------------------------------------------------------------------
@@ -440,23 +409,143 @@ extern "C" int iss_energy_emit(iss_ctx *ctx, int64_t L, int end_state, int out_s
 // path tie closer than ~1e-8 -- the path scores are sums of a handful of constants (-5, -345.39, -23.03, -1e-10)
 // whose distinct combinations are orders of magnitude further apart.  The serial kernel stays available
 // (ISS_B200_VITERBI=serial); the GPU tests compare both with the C oracle, 10 h tracks included.
-constexpr int64_t ECH = 16384;
-
-__global__ void energy_entry_compose_kernel(const double *__restrict__ v0, const double *__restrict__ basis_out,
-                                            int nchunk, double *__restrict__ entry)
+//
+// Chain c is chunk c in steps 1a and 3; chains 2c and 2c + 1 are the basis chains of chunk c in step 1b.
+__global__ void energy_entry_compose_kernel(VitWork w, int n_ech)
 {
     if (threadIdx.x != 0 || blockIdx.x != 0) return;
-    double e0 = v0[0], e1 = v0[1];                               // scores leaving chunk 0 = entering chunk 1
-    for (int c = 1; c < nchunk; ++c) {
-        entry[(c - 1) * MAXK + 0] = e0; entry[(c - 1) * MAXK + 1] = e1;
-        // basis_out slot 2(c-1)+i = scores leaving chunk c when entering in state i with score 0
-        const double *m0 = basis_out + (size_t)(2 * (c - 1)) * MAXK, *m1 = m0 + MAXK;
+    double e0 = w.vout[0], e1 = w.vout[1];                       // scores leaving chunk 0 = entering chunk 1
+    for (int c = 1; c < n_ech; ++c) {
+        w.entry[c * MAXK + 0] = e0; w.entry[c * MAXK + 1] = e1;
+        // vout of chain 2c + i = scores leaving chunk c when entering in state i with score 0
+        const double *m0 = w.vout + (size_t)(2 * c) * MAXK, *m1 = m0 + MAXK;
         const double a0 = e0 + m0[0], b0 = e1 + m1[0], a1 = e0 + m0[1], b1 = e1 + m1[1];
         e0 = (b0 > a0) ? b0 : a0;
         e1 = (b1 > a1) ? b1 : a1;
     }
 }
 
+int energy_viterbi_chunked(const float *d_loge, int64_t L, const double *d_loge_stats, const VitParams &prm,
+                           int out_stride, uint8_t *d_states, void *d_work, cudaStream_t st)
+{
+    const int C = (int)((L + ECH - 1) / ECH);
+    const VitWork w = carve(d_work, L, 1);
+    const int64_t off[2] = {0, L};                               // the backtrack: ONE sequence [0, L)
+    int64_t nc;
+    int rc = upload_offsets(w, off, 1, &nc, st);
+    if (rc != ISS_OK) return rc;
+    std::vector<int64_t> ech_off(C + 1);
+    for (int c = 0; c <= C; ++c) ech_off[c] = std::min<int64_t>((int64_t)c * ECH, L);
+    ISS_CUDA_OK(cudaMemcpyAsync(w.ech_off, ech_off.data(), sizeof(int64_t) * (C + 1), cudaMemcpyHostToDevice, st));
+    std::vector<double> basis((size_t)MAXK * 2 * C, 0.0);
+    for (int c = 0; c < C; ++c) {                                // e_0 = (0, -inf), e_1 = (-inf, 0) in max-plus
+        basis[(size_t)(2 * c) * MAXK + 1] = -INFINITY;
+        basis[(size_t)(2 * c + 1) * MAXK + 0] = -INFINITY;
+    }
+    ISS_CUDA_OK(cudaMemcpyAsync(w.vin, basis.data(), sizeof(double) * basis.size(), cudaMemcpyHostToDevice, st));
+    // 1a. chunk 0, true pass (prior on the first frame), back-pointers stored
+    const VitChains c0 = {w.ech_off, 0, 1, nullptr, w.vout, nullptr, w.bp, 0};
+    viterbi_forward_kernel<2, true><<<1, 32, 0, st>>>(d_loge, d_loge_stats, prm, c0);
+    // 1b. chunks 1..C-1: two basis chains each
+    const VitChains cb = {w.ech_off, 1, 2, w.vin, w.vout, nullptr, nullptr, 0};
+    viterbi_forward_kernel<2, true><<<2 * (C - 1), 32, 0, st>>>(d_loge, d_loge_stats, prm, cb);
+    // 2. entry scores of chunks 1..C-1
+    energy_entry_compose_kernel<<<1, 32, 0, st>>>(w, C);
+    // 3. chunks 1..C-1, true pass from their entry scores
+    const VitChains ct = {w.ech_off, 1, 1, w.entry, nullptr, w.last, w.bp, 0};
+    viterbi_forward_kernel<2, true><<<C - 1, 32, 0, st>>>(d_loge, d_loge_stats, prm, ct);
+    ISS_CUDA_OK(cudaGetLastError());
+    iss_count_launch(4);
+    // 4. backtrack over the whole sequence from the argmax of the last chunk's chain
+    return run_backtrack(w, 1, nc, C - 1, nullptr, out_stride, d_states, st);
+}
+
+}  // namespace
+
+extern "C" int64_t iss_viterbi_work_bytes(int64_t total_steps, int n_seg)
+{
+    if (total_steps < 0 || n_seg < 0) return -1;
+    return (int64_t)carve(nullptr, total_steps, n_seg).bytes;
+}
+
+// ---- partial chains of the energy Viterbi for time-sharded recordings (SURVEY 8(e)) -------------------
+extern "C" int iss_energy_transfer(iss_ctx *ctx, const float *d_loge, int64_t L, const double *d_loge_stats,
+                                   double log_ratio, const double *h_emis, const double *h_trans,
+                                   double *h_matrix, void *d_work, void *stream)
+{
+    ISS_REQUIRE(ctx && d_loge && d_loge_stats && h_emis && h_trans && h_matrix && d_work && L > 0, ISS_ERR_INVALID, "iss_energy_transfer: bad argument");
+    ISS_CUDA_OK(cudaSetDevice(ctx->device));
+    cudaStream_t st = iss_stream(stream);
+    const VitWork w = carve(d_work, L, 1);
+    const int64_t off[2] = {0, L};
+    int64_t nc;
+    int rc = upload_offsets(w, off, 1, &nc, st);
+    if (rc != ISS_OK) return rc;
+    const double NEG_INF = -INFINITY;
+    double vin[2 * MAXK] = {0.0, NEG_INF, 0, 0, NEG_INF, 0.0, 0, 0};      // basis vectors e_0, e_1 (max-plus)
+    ISS_CUDA_OK(cudaMemcpyAsync(w.vin, vin, sizeof(vin), cudaMemcpyHostToDevice, st));
+    const VitChains ch = {w.seq_off, 0, 2, w.vin, w.vout, nullptr, nullptr, 0};
+    viterbi_forward_kernel<2, true><<<2, 32, 0, st>>>(d_loge, d_loge_stats, make_params(2, h_trans, 0.0, h_emis, log_ratio), ch);
+    ISS_CUDA_OK(cudaGetLastError());
+    iss_count_launch();
+    double vout[2 * MAXK];
+    ISS_CUDA_OK(cudaMemcpyAsync(vout, w.vout, sizeof(vout), cudaMemcpyDeviceToHost, st));
+    ISS_CUDA_OK(cudaStreamSynchronize(st));
+    // M[j][i] = score of ending in j having started (before the first frame) in i
+    for (int i = 0; i < 2; ++i) for (int j = 0; j < 2; ++j) h_matrix[j * 2 + i] = vout[i * MAXK + j];
+    return ISS_OK;
+}
+
+extern "C" int iss_energy_forward(iss_ctx *ctx, const float *d_loge, int64_t L, const double *d_loge_stats,
+                                  double log_ratio, const double *h_emis, const double *h_trans, double log_prior,
+                                  const double *h_vin, double *h_vout, uint8_t *h_backmap, void *d_work, void *stream)
+{
+    ISS_REQUIRE(ctx && d_loge && d_loge_stats && h_emis && h_trans && h_vout && h_backmap && d_work && L > 0, ISS_ERR_INVALID, "iss_energy_forward: bad argument");
+    ISS_CUDA_OK(cudaSetDevice(ctx->device));
+    cudaStream_t st = iss_stream(stream);
+    const VitWork w = carve(d_work, L, 1);
+    const int64_t off[2] = {0, L};
+    int64_t nc;
+    int rc = upload_offsets(w, off, 1, &nc, st);
+    if (rc != ISS_OK) return rc;
+    if (h_vin) {
+        double vin[MAXK] = {h_vin[0], h_vin[1], 0, 0};
+        ISS_CUDA_OK(cudaMemcpyAsync(w.vin, vin, sizeof(vin), cudaMemcpyHostToDevice, st));
+    }
+    const VitChains ch = {w.seq_off, 0, 1, h_vin ? w.vin : nullptr, w.vout, w.last, w.bp, 0};
+    viterbi_forward_kernel<2, true><<<1, 32, 0, st>>>(d_loge, d_loge_stats, make_params(2, h_trans, log_prior, h_emis, log_ratio), ch);
+    const unsigned gc = (unsigned)((nc + 127) / 128);
+    viterbi_chunk_map_kernel<<<gc, 128, 0, st>>>(w, 1, nc, h_vin ? 1 : 0);
+    viterbi_compose_kernel<<<1, 32, 0, st>>>(w, nc);
+    ISS_CUDA_OK(cudaGetLastError());
+    iss_count_launch(3);
+    double vout[MAXK];
+    uint8_t m;
+    ISS_CUDA_OK(cudaMemcpyAsync(vout, w.vout, sizeof(vout), cudaMemcpyDeviceToHost, st));
+    ISS_CUDA_OK(cudaMemcpyAsync(&m, w.map, 1, cudaMemcpyDeviceToHost, st));
+    ISS_CUDA_OK(cudaStreamSynchronize(st));
+    h_vout[0] = vout[0]; h_vout[1] = vout[1];
+    h_backmap[0] = m & 3; h_backmap[1] = (m >> 2) & 3;
+    return ISS_OK;
+}
+
+extern "C" int iss_energy_emit(iss_ctx *ctx, int64_t L, int end_state, int out_stride, uint8_t *d_states,
+                               void *d_work, void *stream)
+{
+    ISS_REQUIRE(ctx && d_states && d_work && L > 0 && out_stride >= 1 && end_state >= -1 && end_state < 2, ISS_ERR_INVALID, "iss_energy_emit: bad argument");
+    ISS_CUDA_OK(cudaSetDevice(ctx->device));
+    cudaStream_t st = iss_stream(stream);
+    const VitWork w = carve(d_work, L, 1);                      // iss_energy_forward's tables, already on the device
+    const int64_t nc = (L + CH - 1) / CH;
+    if (end_state >= 0) ISS_CUDA_OK(cudaMemsetAsync(w.last, end_state, 1, st));
+    viterbi_chunk_scan_kernel<<<1, 64, 0, st>>>(w, 1, 0);
+    viterbi_chunk_emit_kernel<<<(unsigned)((nc + 127) / 128), 128, 0, st>>>(w, 1, nc, nullptr, out_stride, d_states);
+    ISS_CUDA_OK(cudaGetLastError());
+    iss_count_launch(3);
+    return ISS_OK;
+}
+
+// ---- whole recordings and CNN segments --------------------------------------------------------------------
 static int g_energy_serial = -1;        // -1: read ISS_B200_VITERBI on first use
 static bool energy_serial()
 {
@@ -464,84 +553,6 @@ static bool energy_serial()
     return g_energy_serial == 1;
 }
 extern "C" int iss_set_energy_viterbi_serial(int serial) { g_energy_serial = serial ? 1 : 0; return ISS_OK; }
-
-static int energy_viterbi_chunked(iss_ctx *ctx, const float *d_loge, int64_t L, const double *d_loge_stats, const VitParams &prm,
-                                  int out_stride, uint8_t *d_states, void *d_work, cudaStream_t st)
-{
-    const int C = (int)((L + ECH - 1) / ECH);
-    // backtrack layout: ONE sequence [0, L)
-    const int64_t off1[2] = {0, L};
-    HostPlan hp1; VitLayout lay1 = {};
-    int rc = make_layout(off1, 1, d_work, hp1, lay1, st);
-    if (rc != ISS_OK) return rc;
-    // forward layout: C segments over the same back-pointer array, tables behind lay1's
-    uint8_t *p = lay1.last + 256;
-    size_t o = 0;
-    std::vector<int64_t> seg(C + 1);
-    for (int c = 0; c <= C; ++c) seg[c] = std::min<int64_t>((int64_t)c * ECH, L);
-    VitLayout lay = lay1;
-    lay.seg_off = reinterpret_cast<int64_t *>(p + o); o = align_up(o + sizeof(int64_t) * (C + 1), 256);
-    lay.last = p + o;                                  o = align_up(o + (size_t)2 * C, 256);
-    double *d_v0 = reinterpret_cast<double *>(p + o);  o += sizeof(double) * MAXK;
-    double *d_basis_in = reinterpret_cast<double *>(p + o);  o += sizeof(double) * MAXK * 2 * C;
-    double *d_basis_out = reinterpret_cast<double *>(p + o); o += sizeof(double) * MAXK * 2 * C;
-    double *d_entry = reinterpret_cast<double *>(p + o);     o += sizeof(double) * MAXK * C;
-    ISS_CUDA_OK(cudaMemcpyAsync(lay.seg_off, seg.data(), sizeof(int64_t) * (C + 1), cudaMemcpyHostToDevice, st));
-    std::vector<double> basis((size_t)MAXK * 2 * C, 0.0);
-    for (int c = 0; c < C; ++c) {                                // e_0 = (0, -inf), e_1 = (-inf, 0) in max-plus
-        basis[(size_t)(2 * c) * MAXK + 1] = -INFINITY;
-        basis[(size_t)(2 * c + 1) * MAXK + 0] = -INFINITY;
-    }
-    ISS_CUDA_OK(cudaMemcpyAsync(d_basis_in, basis.data(), sizeof(double) * basis.size(), cudaMemcpyHostToDevice, st));
-    // 1a. chunk 0, true pass (prior on the first frame), back-pointers stored
-    VitLayout l0 = lay; l0.vin = nullptr; l0.vout = d_v0; l0.alias = 0; l0.store_bp = 1;
-    viterbi_forward_kernel<2, true><<<1, 32, 0, st>>>(d_loge, d_loge_stats, prm, l0);
-    // 1b. chunks 1..C-1: two basis chains each (segment index = 1 + slot / 2 => shift the offset table by one)
-    VitLayout lb = lay; lb.seg_off = lay.seg_off + 1; lb.vin = d_basis_in; lb.vout = d_basis_out; lb.alias = 2; lb.store_bp = 0;
-    viterbi_forward_kernel<2, true><<<2 * (C - 1), 32, 0, st>>>(d_loge, d_loge_stats, prm, lb);
-    // 2. entry scores of chunks 1..C-1
-    energy_entry_compose_kernel<<<1, 32, 0, st>>>(d_v0, d_basis_out, C, d_entry);
-    // 3. chunks 1..C-1, true pass from their entry scores
-    VitLayout lt = lay; lt.seg_off = lay.seg_off + 1; lt.vin = d_entry; lt.vout = nullptr; lt.alias = 0; lt.store_bp = 1;
-    lt.last = lay.last + 1;                                      // last[c] = argmax V at the end of chunk c
-    viterbi_forward_kernel<2, true><<<C - 1, 32, 0, st>>>(d_loge, d_loge_stats, prm, lt);
-    ISS_CUDA_OK(cudaGetLastError());
-    iss_count_launch(4);
-    // 4. backtrack over the whole sequence from the final chunk's argmax
-    lay1.last = lay.last + (C - 1);
-    return run_backtrack(lay1, hp1, 1, out_stride, d_states, st);
-}
-
-extern "C" int64_t iss_viterbi_work_bytes(int64_t total_steps, int n_seg)
-{
-    if (total_steps < 0 || n_seg < 0) return -1;
-    const int64_t nc = total_steps / CH + n_seg + 1;
-    const int64_t chunked = (total_steps / ECH + 2) * 256 + 8192;         // tables of the chunk-parallel energy pass
-    return total_steps + 2 * nc + 3 * (int64_t)sizeof(int64_t) * (n_seg + 1) + n_seg + 9 * 256 + 1024 /* vin/vout/map scratch */ + chunked;
-}
-
-// One serial chain per recording: recording r is loge[h_off[r] .. h_off[r+1]) with statistics stats[2r ..] (stats_stride
-// 2) or the one shared pair (stats_stride 0); every out_stride-th state goes to d_states[h_out_off[r] ..], or to
-// d_states[0 ..] for a single recording (h_out_off == nullptr).
-static int energy_chains(iss_ctx *ctx, const float *d_loge, const int64_t *h_off, int n_rec, const double *d_loge_stats,
-                         int stats_stride, const VitParams &prm, int out_stride, const int64_t *h_out_off, uint8_t *d_states,
-                         void *d_work, cudaStream_t st)
-{
-    HostPlan hp; VitLayout lay = {};
-    int rc = make_layout(h_off, n_rec, d_work, hp, lay, st);
-    if (rc != ISS_OK) return rc;
-    lay.store_bp = 1;
-    lay.stats_stride = stats_stride;
-    if (h_out_off) {
-        int64_t *d_out_off = reinterpret_cast<int64_t *>(lay.last + align_up((size_t)n_rec, 256));
-        ISS_CUDA_OK(cudaMemcpyAsync(d_out_off, h_out_off, sizeof(int64_t) * n_rec, cudaMemcpyHostToDevice, st));
-        lay.out_off = d_out_off;
-    }
-    viterbi_forward_kernel<2, true><<<n_rec, 32, 0, st>>>(d_loge, d_loge_stats, prm, lay);
-    ISS_CUDA_OK(cudaGetLastError());
-    iss_count_launch();
-    return run_backtrack(lay, hp, n_rec, out_stride, d_states, st);
-}
 
 extern "C" int iss_energy_viterbi(iss_ctx *ctx, const float *d_loge, int64_t L, const double *d_loge_stats,
                                   double log_ratio, const double *h_emis, const double *h_trans,
@@ -554,11 +565,10 @@ extern "C" int iss_energy_viterbi(iss_ctx *ctx, const float *d_loge, int64_t L, 
     ISS_REQUIRE(d_loge && d_loge_stats && d_states && d_work, ISS_ERR_INVALID, "iss_energy_viterbi: NULL buffer");
     ISS_CUDA_OK(cudaSetDevice(ctx->device));
     cudaStream_t st = iss_stream(stream);
-    VitParams prm = {};
-    fill_energy_params(prm, h_emis, h_trans, log_prior, log_ratio);
-    if (!energy_serial() && L >= 4 * ECH) return energy_viterbi_chunked(ctx, d_loge, L, d_loge_stats, prm, out_stride, d_states, d_work, st);
+    const VitParams prm = make_params(2, h_trans, log_prior, h_emis, log_ratio);
+    if (!energy_serial() && L >= 4 * ECH) return energy_viterbi_chunked(d_loge, L, d_loge_stats, prm, out_stride, d_states, d_work, st);
     const int64_t off[2] = {0, L};
-    return energy_chains(ctx, d_loge, off, 1, d_loge_stats, 0, prm, out_stride, nullptr, d_states, d_work, st);
+    return decode_sequences<2, true>(d_loge, off, 1, d_loge_stats, 0, prm, out_stride, nullptr, d_states, d_work, st);
 }
 
 extern "C" int iss_energy_viterbi_multi(iss_ctx *ctx, const float *d_loge, const int64_t *h_loge_off, int n_rec,
@@ -578,9 +588,8 @@ extern "C" int iss_energy_viterbi_multi(iss_ctx *ctx, const float *d_loge, const
     ISS_REQUIRE(d_loge && d_loge_stats && d_states && d_work, ISS_ERR_INVALID, "iss_energy_viterbi_multi: NULL buffer");
     ISS_CUDA_OK(cudaSetDevice(ctx->device));
     cudaStream_t st = iss_stream(stream);
-    VitParams prm = {};
-    fill_energy_params(prm, h_emis, h_trans, log_prior, log_ratio);
-    return energy_chains(ctx, d_loge, h_loge_off, n_rec, d_loge_stats, 2, prm, out_stride, h_out_off, d_states, d_work, st);
+    return decode_sequences<2, true>(d_loge, h_loge_off, n_rec, d_loge_stats, 2, make_params(2, h_trans, log_prior, h_emis, log_ratio),
+                                     out_stride, h_out_off, d_states, d_work, st);
 }
 
 extern "C" int iss_viterbi_segments(iss_ctx *ctx, const float *d_probs, int K, const int64_t *h_seg_off,
@@ -593,20 +602,9 @@ extern "C" int iss_viterbi_segments(iss_ctx *ctx, const float *d_probs, int K, c
     ISS_REQUIRE(d_probs && d_states && d_work, ISS_ERR_INVALID, "iss_viterbi_segments: NULL buffer");
     ISS_CUDA_OK(cudaSetDevice(ctx->device));
     cudaStream_t st = iss_stream(stream);
-    HostPlan hp; VitLayout lay = {};
-    int rc = make_layout(h_seg_off, n_seg, d_work, hp, lay, st);
-    if (rc != ISS_OK) return rc;
-    lay.store_bp = 1;
-    VitParams prm = {};
-    for (int i = 0; i < K; ++i) for (int j = 0; j < K; ++j) prm.A[i][j] = h_trans[i * K + j];
-    prm.prior = log_prior;
-    // shift the views so that segment offsets index d_probs rows directly
-    if (K == 2) viterbi_forward_kernel<2, false><<<n_seg, 32, 0, st>>>(d_probs, nullptr, prm, lay);
-    else if (K == 3) viterbi_forward_kernel<3, false><<<n_seg, 32, 0, st>>>(d_probs, nullptr, prm, lay);
-    else viterbi_forward_kernel<4, false><<<n_seg, 32, 0, st>>>(d_probs, nullptr, prm, lay);
-    ISS_CUDA_OK(cudaGetLastError());
-    iss_count_launch();
-    return run_backtrack(lay, hp, n_seg, 1, d_states, st);
+    const VitParams prm = make_params(K, h_trans, log_prior, nullptr, 0.0);
+    auto decode = K == 2 ? decode_sequences<2, false> : K == 3 ? decode_sequences<3, false> : decode_sequences<4, false>;
+    return decode(d_probs, h_seg_off, n_seg, nullptr, 0, prm, 1, nullptr, d_states, d_work, st);
 }
 
 // ---- online decoding of live streams (stream.py) ----------------------------------------------------------------
@@ -641,24 +639,7 @@ viterbi_online_kernel(const float *__restrict__ src, const double *__restrict__ 
     double V[K];
 #pragma unroll
     for (int j = 0; j < K; ++j) V[j] = start ? 0.0 : scores[c.slot * MAXK + j];
-
-    for (int64_t base = 0; base < c.n; base += 32) {
-        const int64_t t = base + lane;
-        double e[K];
-#pragma unroll
-        for (int j = 0; j < K; ++j) e[j] = 0.0;
-        if (t < c.n) load_emissions<K, ENERGY>(src, c.src + t, thr, prm, e);
-        const int nstep = (int)min((int64_t)32, c.n - base);
-        unsigned mybp = 0;
-        for (int s = 0; s < nstep; ++s) {
-            double es[K];
-#pragma unroll
-            for (int j = 0; j < K; ++j) es[j] = __shfl_sync(0xffffffffu, e[j], s);
-            const unsigned bp = vit_step<K, ENERGY>(V, es, prm, start && base + s == 0);
-            if (lane == s) mybp = bp;
-        }
-        if (t < c.n) h[c.pend + t] = (uint8_t)mybp;
-    }
+    forward_steps<K, ENERGY>(src, c.src, c.n, thr, prm, start, V, [&](int64_t t, unsigned b) { h[c.pend + t] = (uint8_t)b; });
     __syncwarp();                                      // the lanes' back-pointer stores are visible to lane 0
 
     const int64_t P = c.pend + c.n;                    // undecided steps: h[0 .. P)
@@ -750,12 +731,7 @@ extern "C" int iss_viterbi_online(iss_ctx *ctx, int K, int n_chain, const int64_
     cudaStream_t st = iss_stream(stream);
     OnlineChain *d_chains = reinterpret_cast<OnlineChain *>(d_work);
     ISS_CUDA_OK(cudaMemcpyAsync(d_chains, h_chains, sizeof(OnlineChain) * n_chain, cudaMemcpyHostToDevice, st));
-    VitParams prm = {};
-    if (energy) fill_energy_params(prm, h_emis, h_trans, log_prior, log_ratio);
-    else {
-        for (int i = 0; i < K; ++i) for (int j = 0; j < K; ++j) prm.A[i][j] = h_trans[i * K + j];
-        prm.prior = log_prior;
-    }
+    const VitParams prm = make_params(K, h_trans, log_prior, h_emis, log_ratio);
     if (energy) launch_online<2, true>(n_chain, st, d_src, d_stats, prm, d_chains, d_scores, d_hist, hist_cap, d_out, d_ndec);
     else if (K == 2) launch_online<2, false>(n_chain, st, d_src, nullptr, prm, d_chains, d_scores, d_hist, hist_cap, d_out, d_ndec);
     else if (K == 3) launch_online<3, false>(n_chain, st, d_src, nullptr, prm, d_chains, d_scores, d_hist, hist_cap, d_out, d_ndec);

@@ -201,6 +201,12 @@ def loge_stats(ctx, loge, stream=None):
 _EMIS = np.log(np.array([1 - 1e-10, 1e-10]))          # pred2logemission, viterbi_utils.py:29-34
 
 
+def _energy_consts(energy_ratio):
+    """(transition matrix, prior log(1/2), log(energy_ratio)) of the energy Viterbi (segmenter.py:69-73)."""
+    trans = np.ascontiguousarray(log_trans_exp(150, cost0=-5), dtype=np.float64)
+    return trans, float(np.log(np.ones(2) / 2)[0]), float(np.log(energy_ratio))
+
+
 def energy_viterbi(ctx, loge, stats, energy_ratio, out_stride=2, stream=None):
     """``_energy_activity(loge, ratio)[::out_stride]`` (segmenter.py:69-73,262) -> CUDA uint8."""
     L = loge.numel()
@@ -210,9 +216,8 @@ def energy_viterbi(ctx, loge, stats, energy_ratio, out_stride=2, stream=None):
         return states
     lib = _lib.load()
     work = ctx.workspace('vit_energy', lib.iss_viterbi_work_bytes(L, 1))
-    trans = np.ascontiguousarray(log_trans_exp(150, cost0=-5), dtype=np.float64)
-    prior = float(np.log(np.ones(2) / 2)[0])
-    _lib.check(lib.iss_energy_viterbi(ctx.handle, _lib.ptr(loge), L, _lib.ptr(stats), float(np.log(energy_ratio)),
+    trans, prior, lr = _energy_consts(energy_ratio)
+    _lib.check(lib.iss_energy_viterbi(ctx.handle, _lib.ptr(loge), L, _lib.ptr(stats), lr,
                                       _lib.ptr(_EMIS), _lib.ptr(trans), prior, int(out_stride),
                                       _lib.ptr(states), _lib.ptr(work), _stream_ptr(loge.device, stream)),
                'iss_energy_viterbi')
@@ -255,11 +260,6 @@ def viterbi_segments(ctx, probs, seg_off, trans, stream=None):
 
 
 # ---- partial energy chains for time-sharded recordings (shard.py) ---------------------------------
-def _energy_consts(energy_ratio):
-    trans = np.ascontiguousarray(log_trans_exp(150, cost0=-5), dtype=np.float64)
-    return trans, float(np.log(np.ones(2) / 2)[0]), float(np.log(energy_ratio))
-
-
 def energy_transfer(ctx, loge, stats, energy_ratio, stream=None):
     """2x2 max-plus transfer matrix (numpy float64, M[j, i]) of this slice of the energy chain."""
     lib = _lib.load()
