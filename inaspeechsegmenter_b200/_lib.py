@@ -35,9 +35,10 @@ LAYER_CONV2D, LAYER_DENSE, LAYER_MAXPOOL = 1, 2, 3
 F_BIAS, F_AFFINE_PRE, F_RELU, F_AFFINE_POST, F_SOFTMAX, F_SIGMOID = 1, 2, 4, 8, 16, 32
 PCM_F32, PCM_S16 = 0, 1
 RESAMPLE_END = 1                      # ISS_RESAMPLE_END
+VBX_END = 1                           # ISS_VBX_END
 FFT_FP32, FFT_FP64 = 0, 1
 GEMM_FP32, GEMM_TC_TS, GEMM_TC_F16 = 0, 2, 3     # fp32 CUDA cores | 3xTF32 wgmma | fp16-split wgmma (default)
-ABI_VERSION = 7                       # == ISS_ABI_VERSION in include/iss_b200.h
+ABI_VERSION = 8                       # == ISS_ABI_VERSION in include/iss_b200.h
 
 # name -> (restype, argtypes); must list every symbol include/iss_b200.h declares
 _vp, _i, _i64, _d = _c.c_void_p, _c.c_int, _c.c_int64, _c.c_double
@@ -78,6 +79,9 @@ SIGNATURES = {
     'iss_vbx_work_bytes': (_i64, [_i64]),
     'iss_vbx_features': (_i, [_vp, _vp, _i, _i64, _vp, _vp, _vp, _vp]),
     'iss_vbx_features_multi': (_i, [_vp, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp]),
+    'iss_vbx_fbank_window_multi': (_i, [_vp, _i, _vp, _vp, _vp, _i, _vp, _vp]),
+    'iss_vbx_cmvn_window_multi': (_i, [_vp, _i, _vp, _vp, _vp, _vp]),
+    'iss_dither_mt19937_multi': (_i, [_vp, _i, _vp, _vp, _i64, _vp, _vp]),
     'iss_resample_num_frames': (_i64, [_i64, _i]),
     'iss_resample_upload_taps': (_i, [_vp, _i, _vp, _i64]),
     'iss_resample_release_taps': (_i, [_vp, _i]),

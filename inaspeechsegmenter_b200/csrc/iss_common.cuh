@@ -62,8 +62,8 @@ struct iss_ctx {
     int64_t partials_cap;        // in tiles
     void *d_recs;                // per-recording table of a features call (feat_sidekit.cu)
     int64_t recs_cap;            // in entries
-    void *d_vbx_recs;            // per-recording table of a VBx features call (feat_vbx.cu)
-    int64_t vbx_recs_cap;        // in entries
+    void *d_vbx_recs;            // record table of a VBx features or dither call (feat_vbx.cu)
+    int64_t vbx_recs_cap;        // in bytes
     void *resample;              // tap tables and recording table of the resampler (resample.cu)
 };
 

@@ -144,6 +144,10 @@ class MlpModel:
 
     def predict(self, x, **_):
         """x: [n, in_dim] numpy or CUDA tensor -> numpy float32 [n, out_dim] (keras predict contract)."""
+        return self.forward(x).cpu().numpy()
+
+    def forward(self, x):
+        """predict without the copy back: a CUDA float32 [n, out_dim] tensor."""
         t = x if isinstance(x, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(x, dtype=np.float32))
         t = t.to(self.ctx.device).contiguous()
         if t.data_ptr() % 16:                       # a view at an odd offset: iss_mlp_forward needs 16-byte rows
@@ -155,7 +159,7 @@ class MlpModel:
             work = self.ctx.workspace('mlp', lib.iss_mlp_workspace_bytes(self.handle, n))
             _lib.check(lib.iss_mlp_forward(self.ctx.handle, self.handle, _lib.ptr(t), n, _lib.ptr(y), _lib.ptr(work),
                                            work.numel(), _stream_ptr(self.ctx.device)), 'iss_mlp_forward')
-        return y.cpu().numpy()
+        return y
 
     def close(self):
         if self.handle:

@@ -139,7 +139,9 @@ class LiveStreams:
     in this call}; ``end(keys)`` returns {key: its remaining segments} and frees the keys; ``decided_until(key)`` is the
     time (s) up to which the stream's labels are final."""
 
-    def __init__(self, seg, calibration_sec=60.0, backend=None):
+    def __init__(self, seg, calibration_sec=60.0, backend=None, observer=None):
+        """``observer``, if given, is called as observer({key: chunk}) with the 16 kHz chunk of every stream in each
+        device pass, before the pass (what ``vfs_stream.LiveScores`` continues its own pipeline from)."""
         if not calibration_sec >= 1.0:
             raise ValueError('calibration_sec must be >= 1.0 (got %r): a stream must hold 68 frames before its '
                              'labels can be decided' % (calibration_sec,))
@@ -148,6 +150,7 @@ class LiveStreams:
         self.vad_labels = seg.vad.outlabels
         self.gender_labels = seg.gender.outlabels if seg.detect_gender else None
         self.backend = backend if backend is not None else CudaBackend(seg)
+        self.observer = observer
         self.streams = {}
         self._free_sids, self._next_sid = [], 0
         self._failed = None            # the error of a call that stopped part way: the object is no longer usable
@@ -266,6 +269,8 @@ class LiveStreams:
 
     def _run(self, chunks, ending):
         be = self.backend
+        if self.observer is not None and chunks:
+            self.observer({st.key: c for st, c in chunks.items()})
         for st, c in chunks.items():
             st.samples += len(c)
         keep = {st.sid: st.R0 for st in self.streams.values()}

@@ -250,11 +250,16 @@ class B200BackendExtractor(VBxExtractor):
         """On the fp16-split engine, a non-finite embedding means an activation left the fp16 range (|x| < 65504 in the
         split-half words between its layers): that is an error, not a window to drop.  The fp32-range engines keep
         the reference's drop-with-warning.  `what` names the recording in the message."""
-        if _lib.load().iss_get_gemm_mode() == _lib.GEMM_TC_F16 and not np.isfinite(emb).all():
+        B200BackendExtractor.check_finite(bool(np.isfinite(emb).all()), what)
+        return emb
+
+    @staticmethod
+    def check_finite(all_finite, what=''):
+        """_check_range's error, from whether every x-vector of a call was finite."""
+        if _lib.load().iss_get_gemm_mode() == _lib.GEMM_TC_F16 and not all_finite:
             raise _lib.IssError('B200BackendExtractor: the ResNet returned non-finite x-vectors%s: an activation left the '
                                 'fp16 range of the default fp16-split GEMM engine; run with ISS_B200_GEMM=tc_ts '
                                 '(3xTF32, fp32 range)' % what)
-        return emb
 
     def get_embedding(self, fea):
         """OnnxBackendExtractor.get_embedding contract (vbx_segmenter.py:262-266): fea [T, 64] -> [256]."""
@@ -334,20 +339,19 @@ def is_mid_speech(start, stop, speech):
     return any(b < m < e for b, e in speech)
 
 
-def add_needed_vectors(xvectors, t_mid):
-    """Keep at least 50 % of the windows whose midpoint is in speech (:40-52): when the
-    overlap threshold removed too many, the windows are taken back in decreasing overlap order.
-    (The reference sorts a ragged object array and reads ``Segment.stop``, which pyannote's Segment
-    does not define; this implements the documented intent with the same selection rule: sort by
-    overlap ratio descending, skip the first len(xvectors) entries, take the next ``diff``.)"""
-    min_pred = round(0.5 * len(t_mid))
-    if len(xvectors) < min_pred:
-        order = np.argsort(np.array([t[0] for t in t_mid], dtype=np.float64))[::-1]
-        ranked = [t_mid[i] for i in order]
-        diff = min_pred - len(xvectors)
-        for _, k, (s0, s1), x in ranked[len(xvectors):len(xvectors) + diff]:
-            xvectors.append((k, (s0, s1), x))
-    return xvectors
+def select_windows(ratios, vad_thresh):
+    """The windows the score keeps, as indices into `ratios` (the speech-overlap ratios of the windows whose midpoint
+    is in speech, in window order), in the order the score takes them: those with ratio >= vad_thresh, then, when
+    fewer than 50 % of the windows were kept, the others in decreasing overlap order up to that share (add_needed_vectors,
+    :40-52).  (The reference sorts a ragged object array and reads ``Segment.stop``, which pyannote's Segment does not
+    define; this implements the documented intent with the same selection rule: sort by overlap ratio descending,
+    skip the first len(kept) entries, take the next ``diff``.)"""
+    kept = [i for i, r in enumerate(ratios) if r >= vad_thresh]
+    min_pred = round(0.5 * len(ratios))
+    if len(kept) < min_pred:
+        order = np.argsort(np.array(ratios, dtype=np.float64))[::-1]
+        kept += [int(i) for i in order[len(kept):min_pred]]
+    return kept
 
 
 def get_femininity_score(g_preds):
@@ -357,6 +361,15 @@ def get_femininity_score(g_preds):
     for start, stop, p in g_preds:
         by_segment[(start, stop)] = bool(np.all(np.asarray(p) >= 0.5))
     return sum(by_segment.values()) / len(by_segment)
+
+
+def score_kept(segs, preds):
+    """(score, nb_vectors) of the kept windows' (start, stop) and their MLP output rows, as __call__ forms them
+    (:188-202); ZeroDivisionError when no window was kept."""
+    if len(preds) > 1:
+        preds = np.squeeze(preds)
+    g = [(seg[0], seg[1], p) for seg, p in zip(segs, preds)]
+    return get_femininity_score(g), len(g)
 
 
 class VoiceFemininityScoring:
@@ -394,14 +407,12 @@ class VoiceFemininityScoring:
 
     def apply_vad(self, xvectors, speech):
         """vbx_segmenter.py:129-145 with `speech` = [(start, end)] of the 'speech' VAD segments."""
-        midpoint_seg, kept = [], []
+        mid, ratios = [], []
         for key, (start, stop), x in xvectors:
             if is_mid_speech(start, stop, speech):
-                ratio = _overlap(start, stop, speech) / (stop - start)
-                if ratio >= self.vad_thresh:
-                    kept.append((key, (start, stop), x))
-                midpoint_seg.append((ratio, key, (start, stop), x))
-        return add_needed_vectors(kept, midpoint_seg)
+                ratios.append(_overlap(start, stop, speech) / (stop - start))
+                mid.append((key, (start, stop), x))
+        return [mid[i] for i in select_windows(ratios, self.vad_thresh)]
 
     def score_signal(self, sig, basename='signal', sample_rate=16000):
         """The body of __call__ on a decoded signal: 16 kHz mono numpy int16 / float, or, at any other ``sample_rate``
@@ -427,10 +438,8 @@ class VoiceFemininityScoring:
         x_vectors = self.apply_vad(x_vectors, speech)
         x = np.asarray([x for _, _, x in x_vectors])
         gender_pred = self.gender_detection_mlp_model.predict(x, verbose=0)
-        if len(gender_pred) > 1:
-            gender_pred = np.squeeze(gender_pred)
-        g = [(seg[0], seg[1], p) for (_, seg, _), p in zip(x_vectors, gender_pred)]
-        return get_femininity_score(g), speech_duration, len(g)
+        score, nb = score_kept([seg for _, seg, _ in x_vectors], gender_pred)
+        return score, speech_duration, nb
 
     def score_signals(self, signals, basename='signal', sample_rates=None):
         """score_signal on each of a list of signals (what score_signal takes, or 1-D int16 / float32 CUDA tensors, read in
@@ -491,14 +500,18 @@ class VoiceFemininityScoring:
         for k, xv in kept.items():
             gender_pred = preds[pos:pos + len(xv)]
             pos += len(xv)
-            if len(gender_pred) > 1:
-                gender_pred = np.squeeze(gender_pred)
-            g = [(seg[0], seg[1], p) for (_, seg, _), p in zip(xv, gender_pred)]
             try:
-                out[k] = (get_femininity_score(g), out[k][1], len(g))
+                score, nb = score_kept([seg for _, seg, _ in xv], gender_pred)
+                out[k] = (score, out[k][1], nb)
             except ZeroDivisionError as e:
                 out[k] = e
         return out
+
+    def stream(self, calibration_sec=60.0):
+        """Extension: live femininity scores of many streams fed chunk by chunk (``vfs_stream.LiveScores``).  The VAD is
+        ``self.vad.stream(calibration_sec)``; a stream's final score is the offline one on its VAD segments."""
+        from .vfs_stream import LiveScores
+        return LiveScores(self, calibration_sec)
 
     def __call__(self, fpath):
         """Voice femininity score of a media file (vbx_segmenter.py:147-202)."""

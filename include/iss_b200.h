@@ -39,7 +39,7 @@ typedef struct iss_mlp iss_mlp;
 
 /* ---- library / context ------------------------------------------------- */
 
-#define ISS_ABI_VERSION 7
+#define ISS_ABI_VERSION 8
 int         iss_version(void);               /* == ISS_ABI_VERSION of the header the library was built from */
 const char *iss_last_error(void);
 /* Creates a context bound to CUDA device `device` (one per host thread that
@@ -300,6 +300,36 @@ int iss_vbx_features(iss_ctx *ctx, const void *d_pcm, int pcm_format, int64_t n_
 int iss_vbx_features_multi(iss_ctx *ctx, int n_rec, const void *const *h_pcm, const int64_t *h_n_samples,
                            int pcm_format, const double *d_dither, float *d_fea, const int64_t *h_fea_off,
                            void *d_work, void *stream);
+/* The same front end over windows of streams fed piece by piece (live streams), in two steps that run the kernels of
+ * iss_vbx_features_multi (which is the window s_base = r_first = r_base = t_first = 0 with ISS_VBX_END of each
+ * recording), so every row equals, bit for bit, the same row of iss_vbx_features on the whole stream.
+ * Raw rows (float64 log-fbank before CMVN), n_rec records of one pcm_format in one launch: record r is the int64 row
+ * h_win[6 r ..] = {s_base, s_known, r_first, rows, raw_off, flags}.  h_pcm[r] and h_dither[r] (DEVICE pointers, the
+ * dither as d_dither above, or NULL for none) hold samples [s_base, s_known) of the stream; raw rows r_first ..
+ * r_first + rows - 1 go to d_raw rows raw_off ...  Row t reads samples max(0, 160 t - 120) .. 160 t + 279 and is final
+ * once 160 t + 280 <= s_known; the mirrored rows past that read around s_known, the stream's last sample, and are
+ * allowed only once it has ended (ISS_VBX_END).  Checked on the host before the launch, ISS_ERR_INVALID with the
+ * record's index: no row reads a sample before s_base; without ISS_VBX_END no row reads a sample at or past s_known;
+ * with it, rows < iss_vbx_num_frames(s_known). */
+#define ISS_VBX_END 1
+int iss_vbx_fbank_window_multi(iss_ctx *ctx, int n_rec, const void *const *h_pcm, const double *const *h_dither,
+                               const int64_t *h_win, int pcm_format, double *d_raw, void *stream);
+/* CMVN rows, n_rec records in one launch: record r is h_win[7 r ..] = {r_base, r_known, t_first, rows, raw_off,
+ * fea_off, flags}: d_raw rows raw_off .. hold raw rows [r_base, r_known) of the stream; feature rows t_first ..
+ * t_first + rows - 1 go to d_fea rows fea_off ...  r_known is the M of the sliding window.  Each row is computed by
+ * replaying its 128-row chunk of the whole-recording grid from the chunk's start, so it is the same sum in the same
+ * order.  Checked on the host: rows < r_known; without ISS_VBX_END, r_known >= 300 and t_first + rows - 1 + 150 <=
+ * r_known (rows whose window can no longer change); the window start of the chunk of t_first is >= r_base. */
+int iss_vbx_cmvn_window_multi(iss_ctx *ctx, int n_rec, const int64_t *h_win, const double *d_raw, float *d_fea,
+                              void *stream);
+/* The dither of d_dither above, drawn on the device for many streams, each from its own MT19937 state, in one launch.
+ * d_state: uint32 [n_slots][625], row s = the 624 key words and the position of numpy's RandomState(3).get_state()
+ * when stream slot s opens; record r = h_rec[3 r ..] = {slot, n, out_off} writes the slot's next n dither values to
+ * d_out[out_off ..] and advances its state, so a stream's values concatenate to 8 * (2 RandomState(3).rand(N) - 1).
+ * A state position that is odd or past 624 is read as 624 (the next draw twists first).  ISS_ERR_INVALID (host check,
+ * no launch) for a slot out of range or drawn twice in one call, or n_slots >= 2^31. */
+int iss_dither_mt19937_multi(iss_ctx *ctx, int n_rec, const int64_t *h_rec, uint32_t *d_state, int64_t n_slots,
+                             double *d_out, void *stream);
 
 /* ---- Resampling to 16 kHz mono -----------------------------------------------
  * No reference counterpart: the reference has ffmpeg decode with `-ar 16000 -ac 1`
