@@ -714,28 +714,45 @@ constexpr int SLAB_MAX_SMEM = MAX_SMEM;
 int slab_rows(int KH, int KW, int W) { return (SLAB_TS + (KH - 1) * W + KW - 1 + 7) & ~7; }
 int slab_smem(int rows, int nbuf, int stages) { return stages * SLAB_B_STAGE + nbuf * 2 * rows * 128 + 1024; }
 
-// one 16-byte chunk of the slab: chunk j of pixel row r (pixel s0 + r) at chunk j ^ (r & 7) of both planes
+// One 16-byte chunk of the slab, chunk j of pixel row r (pixel p = s0 + r = (img * H + ih) * W + iw): slab_load issues
+// the global loads of the chunk's 8 channels (for LD_FIRST the map Y of the pixel's own patch; zeros past the batch),
+// slab_store evaluates, splits and stores them at chunk j ^ (r & 7) of both planes.
+struct SlabRaw {
+    uint4 x[4];                                               // LD_FIRST: Yh (x[0..1]) and Yl (x[2..3]); else x[0..1]
+};
+
 template <int MODE>
-__device__ __forceinline__ void slab_fill_chunk(const ConvArgs &a, const FirstFuse &ff, uint32_t slab_hi, uint32_t slab_lo,
-                                                int64_t s0, int u, int64_t HW, int64_t npix)
+__device__ __forceinline__ void slab_load(const ConvArgs &a, const FirstFuse &ff, int64_t p, int64_t img, int ih, int iw,
+                                          int j, bool ok, SlabRaw &raw)
 {
-    const int r = u >> 3, j = u & 7;
-    const int64_t p = s0 + r;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) raw.x[q] = make_uint4(0u, 0u, 0u, 0u);
+    if (!ok) return;
+    if constexpr (MODE == LD_FIRST) {
+        const int64_t o = (((int64_t)__ldg(ff.row0 + img) - ff.y_f0 + ih) * a.W + iw) * SLAB_C + j * 8;
+        const uint4 *yh = reinterpret_cast<const uint4 *>(ff.Yh + o), *yl = reinterpret_cast<const uint4 *>(ff.Yl + o);
+        raw.x[0] = __ldg(yh); raw.x[1] = __ldg(yh + 1); raw.x[2] = __ldg(yl); raw.x[3] = __ldg(yl + 1);
+    } else {                                                  // NHWC pixel p of the batch is the tall image's pixel p
+        const uint4 *src = reinterpret_cast<const uint4 *>(a.in + p * SLAB_C + j * 8);
+        raw.x[0] = __ldg(src); raw.x[1] = __ldg(src + 1);
+    }
+}
+
+template <int MODE>
+__device__ __forceinline__ void slab_store(const FirstFuse &ff, const SlabRaw &raw, int64_t img, int j, bool ok, uint32_t slab_hi,
+                                           uint32_t slab_lo, int r)
+{
     uint32_t hw[4] = {0u, 0u, 0u, 0u}, lw[4] = {0u, 0u, 0u, 0u};
-    if (p < npix) {
-        if constexpr (MODE == LD_FIRST) {                     // the first layer at pixel p, from the map Y of its own patch
-            const int64_t img = p / HW;
-            const int rem = (int)(p - img * HW);
-            const int ih = rem / a.W, iw = rem - ih * a.W;
-            const int64_t o = (((int64_t)__ldg(ff.row0 + img) - ff.y_f0 + ih) * a.W + iw) * SLAB_C + j * 8;
-            const float4 *yh = reinterpret_cast<const float4 *>(ff.Yh + o), *yl = reinterpret_cast<const float4 *>(ff.Yl + o);
+    if (ok) {
+        if constexpr (MODE == LD_FIRST) {                     // the first layer at the pixel
             const float4 *cf = reinterpret_cast<const float4 *>(ff.coef + img * (3 * SLAB_C) + j * 8);
             float v[8];
 #pragma unroll
             for (int q = 0; q < 2; ++q) {
-                const float4 h4 = __ldg(yh + q), l4 = __ldg(yl + q);
+                const uint4 h4 = raw.x[q], l4 = raw.x[2 + q];
                 const float4 va = __ldg(cf + q), vh = __ldg(cf + SLAB_C / 4 + q), vl = __ldg(cf + 2 * (SLAB_C / 4) + q);
-                const float hv[4] = {h4.x, h4.y, h4.z, h4.w}, lv[4] = {l4.x, l4.y, l4.z, l4.w};
+                const float hv[4] = {__uint_as_float(h4.x), __uint_as_float(h4.y), __uint_as_float(h4.z), __uint_as_float(h4.w)};
+                const float lv[4] = {__uint_as_float(l4.x), __uint_as_float(l4.y), __uint_as_float(l4.z), __uint_as_float(l4.w)};
                 const float al[4] = {va.x, va.y, va.z, va.w}, bh[4] = {vh.x, vh.y, vh.z, vh.w}, bl[4] = {vl.x, vl.y, vl.z, vl.w};
 #pragma unroll
                 for (int e = 0; e < 4; ++e) {
@@ -749,9 +766,8 @@ __device__ __forceinline__ void slab_fill_chunk(const ConvArgs &a, const FirstFu
                 }
             }
             split_f16(v, hw, lw);
-        } else {                                              // NHWC pixel p of the batch is the tall image's pixel p
-            const uint4 *src = reinterpret_cast<const uint4 *>(a.in + p * SLAB_C + j * 8);
-            const uint4 u0 = __ldg(src), u1 = __ldg(src + 1);
+        } else {
+            const uint4 u0 = raw.x[0], u1 = raw.x[1];
             if constexpr (MODE == LD_PACKED) {
                 const uint32_t w[8] = {u0.x, u0.y, u0.z, u0.w, u1.x, u1.y, u1.z, u1.w};
                 words_to_planes(w, hw, lw);
@@ -766,6 +782,37 @@ __device__ __forceinline__ void slab_fill_chunk(const ConvArgs &a, const FirstFu
     const uint32_t dst = (uint32_t)r * 128u + ((uint32_t)(j ^ (r & 7)) << 4);
     sts128(slab_hi + dst, hw[0], hw[1], hw[2], hw[3]);
     sts128(slab_lo + dst, lw[0], lw[1], lw[2], lw[3]);
+}
+
+// (img, ih, iw) of the pixel n rows of the tall image further on (n >= 0)
+__device__ __forceinline__ void slab_step(const ConvArgs &a, int n, int64_t &img, int &ih, int &iw)
+{
+    iw += n;
+    while (iw >= a.W) { iw -= a.W; if (++ih == a.H) { ih = 0; ++img; } }
+}
+
+// The slab of the tile at slot s0, filled by fill thread ft of 96: chunk j = ft % 8 of the pixel rows ft / 8 + 12 i.
+// The thread walks its pixels' (img, ih, iw) from one division per tile instead of dividing the 64-bit pixel index
+// for every row: the fill sets the pace of the layer, and those divisions were most of its dependent instructions.
+// (Keeping two rows' loads in flight instead spills the LD_FIRST producer at 56 registers and was slower.)
+template <int MODE>
+__device__ __forceinline__ void slab_fill(const ConvArgs &a, const FirstFuse &ff, uint32_t slab_hi, uint32_t slab_lo, int rows,
+                                          int64_t s0, int ft, int64_t HW, int64_t n_img)
+{
+    constexpr int STEP = SLAB_FILL_THREADS / 8;                // rows between a thread's rows
+    const int j = ft & 7;
+    int r = ft >> 3;
+    int64_t img = (s0 + r) / HW;
+    const int rem = (int)(s0 + r - img * HW);
+    int ih = rem / a.W, iw = rem - ih * a.W;
+#pragma unroll 1
+    for (; r < rows; r += STEP) {
+        const bool ok0 = img < n_img;
+        SlabRaw raw0;
+        slab_load<MODE>(a, ff, s0 + r, img, ih, iw, j, ok0, raw0);
+        slab_store<MODE>(ff, raw0, img, j, ok0, slab_hi, slab_lo, r);
+        slab_step(a, STEP, img, ih, iw);
+    }
 }
 
 template <int MODE>
@@ -794,7 +841,6 @@ conv_slab_kernel(const ConvArgs a, const FirstFuse ff, const unsigned char *__re
     const int nkb = a.KH * a.KW;                             // one k-block (64 channels) per tap
     const int64_t HW = (int64_t)a.H * a.W;
     const int64_t n_img = a.M / ((int64_t)a.OH * a.OW);
-    const int64_t npix = n_img * HW;
 
     if (wg == 0) {
         // ============================ producer ============================
@@ -817,9 +863,7 @@ conv_slab_kernel(const ConvArgs a, const FirstFuse ff, const unsigned char *__re
             for (int64_t tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
                 mbar_wait(sempty + 8 * b, ph ^ 1);           // both consumers retired their last wgmma on this buffer
                 const uint32_t hi = slab0 + (uint32_t)b * slab_bytes, lo = hi + (uint32_t)rows * 128u;
-#pragma unroll 1
-                for (int u = tid - 32; u < rows * 8; u += SLAB_FILL_THREADS)
-                    slab_fill_chunk<MODE>(a, ff, hi, lo, tile * SLAB_TS, u, HW, npix);
+                slab_fill<MODE>(a, ff, hi, lo, rows, tile * SLAB_TS, tid - 32, HW, n_img);
                 fence_proxy_async();                         // this thread's slab stores, visible to wgmma
                 mbar_arrive(sfull + 8 * b);
                 if (++b == nbuf) { b = 0; ph ^= 1; }
