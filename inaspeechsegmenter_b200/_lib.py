@@ -34,11 +34,12 @@ class LayerDesc(_c.Structure):
 LAYER_CONV2D, LAYER_DENSE, LAYER_MAXPOOL = 1, 2, 3
 F_BIAS, F_AFFINE_PRE, F_RELU, F_AFFINE_POST, F_SOFTMAX, F_SIGMOID = 1, 2, 4, 8, 16, 32
 PCM_F32, PCM_S16 = 0, 1
+PCM_U8, PCM_S24, PCM_S32, PCM_F64 = 2, 3, 4, 5      # WAV encodings the resampler alone reads
 RESAMPLE_END = 1                      # ISS_RESAMPLE_END
 VBX_END = 1                           # ISS_VBX_END
 FFT_FP32, FFT_FP64 = 0, 1
 GEMM_FP32, GEMM_TC_TS, GEMM_TC_F16 = 0, 2, 3     # fp32 CUDA cores | 3xTF32 wgmma | fp16-split wgmma (default)
-ABI_VERSION = 8                       # == ISS_ABI_VERSION in include/iss_b200.h
+ABI_VERSION = 9                      # == ISS_ABI_VERSION in include/iss_b200.h
 
 # name -> (restype, argtypes); must list every symbol include/iss_b200.h declares
 _vp, _i, _i64, _d = _c.c_void_p, _c.c_int, _c.c_int64, _c.c_double

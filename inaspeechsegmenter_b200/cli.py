@@ -28,7 +28,7 @@ def build_parser():
     p.add_argument('-s', '--batch_size', type=int, default=32, help='kept for compatibility (the GPU kernels batch internally)')
     p.add_argument('-d', '--vad_engine', choices=['sm', 'smn'], default='smn')
     p.add_argument('-g', '--detect_gender', choices=['true', 'false'], default='True')
-    p.add_argument('-b', '--ffmpeg_binary', default='ffmpeg', help='ffmpeg binary; "None" disables ffmpeg (16 kHz WAV input only)')
+    p.add_argument('-b', '--ffmpeg_binary', default='ffmpeg', help='ffmpeg binary; "None" disables ffmpeg (WAV input only)')
     p.add_argument('-e', '--export_format', choices=['csv', 'textgrid'], default='csv')
     p.add_argument('-r', '--energy_ratio', default=0.03, type=float)
     p.add_argument('--devices', default='0', help='comma-separated CUDA ordinals; files are dealt round-robin, one process per GPU')
@@ -48,7 +48,7 @@ def main(argv=None):
     args = build_parser().parse_args(argv)
     ffmpeg = args.ffmpeg_binary
     if ffmpeg.lower() == 'none' or ffmpeg == '':
-        print('Disabling ffmpeg. Make sure your audio files are already sampled at 16kHz.')
+        print('Disabling ffmpeg. WAV input only.')
         ffmpeg = None
     input_files = []
     for e in args.input:

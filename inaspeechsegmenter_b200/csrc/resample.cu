@@ -1,7 +1,8 @@
-// resample.cu -- downmix + polyphase FIR resampling of int16 / float32 PCM to 16 kHz mono int16.
+// resample.cu -- downmix + polyphase FIR resampling of PCM (int16, float32, and the WAV encodings unsigned 8-bit,
+// packed 24-bit, int32 and float64) to 16 kHz mono int16.
 //
 // Definition (DESIGN.md "Resampling"): a recording of n frames, C channels at integer rate R is
-//   x[m]  = mean over the C channels of frame m in float64 (int16 s as s / 32768, float32 as is),
+//   x[m]  = mean over the C channels of frame m in float64 (int16 s as s / 32768, float32 as is; pcm_value below),
 //   y[k]  = scipy.signal.resample_poly(x, up, down)[k],  up = 16000 / g, down = R / g, g = gcd(16000, R),
 //         = sum_m x[m] h[k * down + H - m * up]  with h the 2H + 1 taps (H = 10 max(up, down)) of scipy's
 //           default design times up, and x = 0 outside [0, n),
@@ -11,7 +12,8 @@
 //
 // Layout: one CTA owns a tile of consecutive outputs of one record (tiles start at the record's first output k_first).
 // It stages the raw samples of the tile's input span in shared memory with 16-byte loads (scalar loads when the
-// record's base pointer is not 16-byte aligned), downmixes them there into float64, then each thread evaluates
+// record's base pointer is not 16-byte aligned; packed 24-bit samples are staged as bytes and sign-extended in the
+// downmix), downmixes them there into float64, then each thread evaluates
 // its outputs as float64 FMA chains in ascending frame order.  No atomics, and no value depends on the tiling.
 //
 // Windows (live streams): a record's buffer holds frames [f_base, n_known) of its stream, and it computes outputs
@@ -22,7 +24,6 @@
 #include <string.h>
 
 #include <map>
-#include <type_traits>
 #include <vector>
 
 #include "iss_common.cuh"
@@ -55,23 +56,46 @@ struct RsRec {
     int vec_ok;                     // pcm is 16-byte aligned
 };
 
+// A stored sample is UNITS consecutive Units (what the staging loads: bytes for packed 24-bit) in record order.
+template <int PCM> struct PcmIn;
+template <> struct PcmIn<ISS_PCM_F32> { using Unit = float;   static constexpr int UNITS = 1; };
+template <> struct PcmIn<ISS_PCM_S16> { using Unit = int16_t; static constexpr int UNITS = 1; };
+template <> struct PcmIn<ISS_PCM_U8>  { using Unit = uint8_t; static constexpr int UNITS = 1; };
+template <> struct PcmIn<ISS_PCM_S24> { using Unit = uint8_t; static constexpr int UNITS = 3; };
+template <> struct PcmIn<ISS_PCM_S32> { using Unit = int32_t; static constexpr int UNITS = 1; };
+template <> struct PcmIn<ISS_PCM_F64> { using Unit = double;  static constexpr int UNITS = 1; };
+
+// Step 1 of the definition: the stored sample at p as float64.  Every scale is a power of two, so each value is exact.
+template <int PCM>
+__device__ __forceinline__ double pcm_value(const typename PcmIn<PCM>::Unit *p)
+{
+    if constexpr (PCM == ISS_PCM_S16) return (double)p[0] * (1.0 / 32768.0);
+    else if constexpr (PCM == ISS_PCM_U8) return (double)((int)p[0] - 128) * (1.0 / 128.0);
+    else if constexpr (PCM == ISS_PCM_S24)        // little-endian; the shift pair sign-extends bit 23
+        return (double)((int)(((uint32_t)p[0] << 8) | ((uint32_t)p[1] << 16) | ((uint32_t)p[2] << 24)) >> 8) *
+               (1.0 / 8388608.0);
+    else if constexpr (PCM == ISS_PCM_S32) return (double)p[0] * (1.0 / 2147483648.0);
+    else return (double)p[0];                     // float32, float64
+}
+
 template <int PCM>
 __global__ void __launch_bounds__(RS_THREADS)
 resample_kernel(const RsRec *__restrict__ recs, int n_rec, const Phase *__restrict__ phases,
                 const double *__restrict__ taps, int up, int down, int channels, int tile_out, int s_min, int e_max,
                 int span_cap, int16_t *__restrict__ out_all)
 {
-    using Sample = typename std::conditional<PCM == ISS_PCM_S16, int16_t, float>::type;
-    constexpr int VEC = 16 / sizeof(Sample);
+    using Unit = typename PcmIn<PCM>::Unit;
+    constexpr int UNITS = PcmIn<PCM>::UNITS;
+    constexpr int VEC = 16 / sizeof(Unit);
     extern __shared__ __align__(16) unsigned char smem_raw[];
     double *xs = reinterpret_cast<double *>(smem_raw);                                   // [span_cap] downmixed frames
-    Sample *raw = reinterpret_cast<Sample *>(smem_raw + (((size_t)span_cap * sizeof(double) + 15) & ~(size_t)15));
+    Unit *raw = reinterpret_cast<Unit *>(smem_raw + (((size_t)span_cap * sizeof(double) + 15) & ~(size_t)15));
     const int tid = threadIdx.x;
 
     int lo = 0, hi = n_rec;                                      // recs[lo].tile_off <= blockIdx.x < recs[hi].tile_off
     while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (recs[mid].tile_off <= (int64_t)blockIdx.x) lo = mid; else hi = mid; }
     const RsRec &rec = recs[lo];
-    const Sample *pcm = reinterpret_cast<const Sample *>(rec.pcm);
+    const Unit *pcm = reinterpret_cast<const Unit *>(rec.pcm);
     const int64_t fb = rec.f_base, n = rec.n_known;
     const int64_t k0 = rec.k_first + ((int64_t)blockIdx.x - rec.tile_off) * tile_out;
     const int nk = (int)min((int64_t)tile_out, rec.k_first + rec.n_out - k0);
@@ -79,11 +103,12 @@ resample_kernel(const RsRec *__restrict__ recs, int n_rec, const Phase *__restri
     const int64_t f_hi = ((k0 + nk - 1) * down) / up + e_max;
     const int span = (int)(f_hi - f_lo);                                      // <= span_cap
 
-    // ---- raw samples of frames [max(f_lo, f_base), min(f_hi, n)) ----
+    // ---- raw samples of frames [max(f_lo, f_base), min(f_hi, n)); vector loads stay inside the record, since its base
+    // is 16-byte aligned and they end at or before unit e_hi ----
     const int64_t g_lo = max(f_lo, fb), g_hi = min(f_hi, n);
-    int64_t rb = 0;                                              // raw[i] holds sample element rb + i of pcm
+    int64_t rb = 0;                                              // raw[i] holds unit rb + i of pcm
     if (g_lo < g_hi) {
-        const int64_t e_lo = (g_lo - fb) * channels, e_hi = (g_hi - fb) * channels;
+        const int64_t e_lo = (g_lo - fb) * channels * UNITS, e_hi = (g_hi - fb) * channels * UNITS;
         if (rec.vec_ok) {
             rb = e_lo & ~(int64_t)(VEC - 1);
             const int64_t v_hi = e_hi & ~(int64_t)(VEC - 1);
@@ -100,14 +125,13 @@ resample_kernel(const RsRec *__restrict__ recs, int n_rec, const Phase *__restri
     __syncthreads();
 
     // ---- downmix: mean over the channels in float64, channel order; zeros outside the recording ----
-    const double inv = (PCM == ISS_PCM_S16) ? 1.0 / 32768.0 : 1.0;
     for (int i = tid; i < span; i += RS_THREADS) {
         const int64_t f = f_lo + i;
         double v = 0.0;
         if (f >= fb && f < n) {
-            const Sample *p = raw + ((f - fb) * channels - rb);
+            const Unit *p = raw + ((f - fb) * channels * UNITS - rb);
             double s = 0.0;
-            for (int c = 0; c < channels; ++c) s += (double)p[c] * inv;
+            for (int c = 0; c < channels; ++c) s += pcm_value<PCM>(p + c * UNITS);
             v = s / (double)channels;
         }
         xs[i] = v;
@@ -238,12 +262,25 @@ extern "C" int iss_resample_release_taps(iss_ctx *ctx, int rate)
     return ISS_OK;
 }
 
-// Largest power-of-two tile (outputs per CTA) whose staged span fits the shared-memory budget.
-static void tile_for(const ResampleTable &t, int channels, int itemsize, int *tile, int *span_cap, size_t *smem)
+// Bytes of one stored sample of a pcm_format check_call accepts.
+static int sample_bytes(int pcm_format)
+{
+    switch (pcm_format) {
+    case ISS_PCM_U8: return 1;
+    case ISS_PCM_S16: return 2;
+    case ISS_PCM_S24: return 3;
+    case ISS_PCM_F64: return 8;
+    default: return 4;                                   // float32, int32
+    }
+}
+
+// Largest power-of-two tile (outputs per CTA) whose staged span fits the shared-memory budget.  With 8 channels of
+// float64, the widest frame, every rate from 8 to 192 kHz fits at a tile of 64 or more; run_records checks the fit.
+static void tile_for(const ResampleTable &t, int channels, int bytes, int *tile, int *span_cap, size_t *smem)
 {
     for (int to = RS_MAX_TILE;; to >>= 1) {
         const int64_t span = ((int64_t)(to - 1) * t.down + t.up - 1) / t.up + 1 + (t.e_max - t.s_min);
-        const int64_t raw = ((span * channels + 16 / itemsize) * itemsize + 15) & ~(int64_t)15;   // + one vector of slack
+        const int64_t raw = (span * channels * bytes + 16 + 15) & ~(int64_t)15;           // + one vector of slack
         const int64_t bytes = ((span * (int64_t)sizeof(double) + 15) & ~(int64_t)15) + raw;
         if (bytes <= RS_SMEM_BUDGET || to == RS_MIN_TILE) {
             *tile = to; *span_cap = (int)span; *smem = (size_t)bytes;
@@ -270,7 +307,9 @@ static int check_call(iss_ctx *ctx, const char *fn, int n_rec, const void *args,
                       const ResampleTable **out)
 {
     ISS_REQUIRE(ctx, ISS_ERR_INVALID, "%s: ctx is NULL", fn);
-    ISS_REQUIRE(pcm_format == ISS_PCM_F32 || pcm_format == ISS_PCM_S16, ISS_ERR_INVALID, "bad pcm_format %d", pcm_format);
+    ISS_REQUIRE(pcm_format == ISS_PCM_F32 || pcm_format == ISS_PCM_S16 || pcm_format == ISS_PCM_U8 ||
+                pcm_format == ISS_PCM_S24 || pcm_format == ISS_PCM_S32 || pcm_format == ISS_PCM_F64,
+                ISS_ERR_INVALID, "bad pcm_format %d", pcm_format);
     ISS_REQUIRE(channels >= 1 && channels <= RS_MAX_CHANNELS, ISS_ERR_INVALID,
                 "%s: %d channels outside [1, %d]", fn, channels, RS_MAX_CHANNELS);
     ISS_REQUIRE(rate_ok(rate), ISS_ERR_INVALID, "%s: rate %d outside [%d, %d]", fn, rate, RS_MIN_RATE, RS_MAX_RATE);
@@ -289,10 +328,10 @@ static int run_records(iss_ctx *ctx, const char *fn, const ResampleTable &t, std
     ResampleState *s = rs_state(ctx);
     ISS_CUDA_OK(cudaSetDevice(ctx->device));
     cudaStream_t st = iss_stream(stream);
-    const int itemsize = pcm_format == ISS_PCM_S16 ? 2 : 4;
     int tile, span_cap;
     size_t smem;
-    tile_for(t, channels, itemsize, &tile, &span_cap, &smem);
+    tile_for(t, channels, sample_bytes(pcm_format), &tile, &span_cap, &smem);
+    ISS_REQUIRE(smem <= (size_t)RS_SMEM_BUDGET, ISS_ERR_INVALID, "%s: staged span of %zu bytes over the budget", fn, smem);
     const int n_rec = (int)recs.size() - 1;
     int64_t ntiles = 0;
     for (int i = 0; i < n_rec; ++i) {
@@ -315,9 +354,14 @@ static int run_records(iss_ctx *ctx, const char *fn, const ResampleTable &t, std
     }
     const RsRec *d_recs = reinterpret_cast<const RsRec *>(s->d_recs);
     ISS_CUDA_OK(cudaMemcpyAsync(s->d_recs, recs.data(), sizeof(RsRec) * (n_rec + 1), cudaMemcpyHostToDevice, st));
-    return pcm_format == ISS_PCM_S16
-               ? launch_resample<ISS_PCM_S16>(t, d_recs, n_rec, ntiles, channels, tile, span_cap, smem, d_out, st)
-               : launch_resample<ISS_PCM_F32>(t, d_recs, n_rec, ntiles, channels, tile, span_cap, smem, d_out, st);
+    switch (pcm_format) {
+    case ISS_PCM_S16: return launch_resample<ISS_PCM_S16>(t, d_recs, n_rec, ntiles, channels, tile, span_cap, smem, d_out, st);
+    case ISS_PCM_U8: return launch_resample<ISS_PCM_U8>(t, d_recs, n_rec, ntiles, channels, tile, span_cap, smem, d_out, st);
+    case ISS_PCM_S24: return launch_resample<ISS_PCM_S24>(t, d_recs, n_rec, ntiles, channels, tile, span_cap, smem, d_out, st);
+    case ISS_PCM_S32: return launch_resample<ISS_PCM_S32>(t, d_recs, n_rec, ntiles, channels, tile, span_cap, smem, d_out, st);
+    case ISS_PCM_F64: return launch_resample<ISS_PCM_F64>(t, d_recs, n_rec, ntiles, channels, tile, span_cap, smem, d_out, st);
+    default: return launch_resample<ISS_PCM_F32>(t, d_recs, n_rec, ntiles, channels, tile, span_cap, smem, d_out, st);
+    }
 }
 
 extern "C" int iss_resample_to16k_multi(iss_ctx *ctx, int n_rec, const void *const *h_pcm, const int64_t *h_n_frames,

@@ -9,33 +9,95 @@ float32 / float64) with soundfile's integer scaling (value / 2**(bits-1)).
 Additionally ``return_int16=True`` hands back the raw int16 samples when the
 source is PCM16 so that the device front-end can ingest 2 bytes/sample (the
 conversion s/32768 then happens in the kernel, bit-identical to soundfile's).
+
+``wav_data`` reads a WAV header alone: with ffmpeg disabled, a WAV that is not
+16 kHz mono is uploaded as stored and decoded by the device resampler
+(segmenter._media2feats).
 """
+import mmap
 import struct
 import subprocess
+from collections import namedtuple
 from tempfile import TemporaryFile
 
 import numpy as np
 
 
-def _parse_wav(raw):
+def _wav_chunks(raw):
+    """(fmt, start, stop) of a RIFF/WAVE image (bytes, or an mmap: only the fmt chunk is copied): the fmt fields
+    (tag, channels, rate, byte rate, block align, bits) and the byte range of the data chunk, cut at the end of raw."""
     if raw[:4] != b'RIFF' or raw[8:12] != b'WAVE':
         raise ValueError('not a RIFF/WAVE file')
     pos, fmt, data = 12, None, None
     while pos + 8 <= len(raw):
         cid = raw[pos:pos + 4]
         size = struct.unpack('<I', raw[pos + 4:pos + 8])[0]
-        body = raw[pos + 8:pos + 8 + size]
         if cid == b'fmt ':
+            body = raw[pos + 8:pos + 8 + size]
             fmt = struct.unpack('<HHIIHH', body[:16])
             if fmt[0] == 0xFFFE and len(body) >= 26:        # WAVE_FORMAT_EXTENSIBLE: sub-format tag
                 fmt = (struct.unpack('<H', body[24:26])[0],) + fmt[1:]
         elif cid == b'data':
-            data = body if size != 0xFFFFFFFF else raw[pos + 8:]     # ffmpeg pipes write size -1
+            stop = len(raw) if size == 0xFFFFFFFF else min(pos + 8 + size, len(raw))   # ffmpeg pipes write size -1
+            data = (pos + 8, stop)
             break
         pos += 8 + size + (size & 1)
     if fmt is None or data is None:
         raise ValueError('missing fmt/data chunk')
-    return fmt, data
+    return (fmt,) + data
+
+
+def _parse_wav(raw):
+    fmt, start, stop = _wav_chunks(raw)
+    return fmt, raw[start:stop]
+
+
+# encoding of a WAV by (format tag, container bits): what read_wav decodes, named as resample.PCM_FORMATS
+_ENCODINGS = {(1, 8): 'u8', (1, 16): 's16', (1, 24): 's24', (1, 32): 's32', (3, 32): 'f32', (3, 64): 'f64'}
+BYTES = {'u8': 1, 's16': 2, 's24': 3, 's32': 4, 'f32': 4, 'f64': 8}
+
+
+class WavData(namedtuple('WavData', 'path encoding channels rate frames start stop')):
+    """The layout of a WAV file (wav_data): its samples are the bytes [start, stop) of the file, `frames` frames of
+    `channels` interleaved samples of `encoding` at `rate` Hz."""
+
+    @property
+    def shape(self):
+        """[frames, channels, bytes per sample]: the stored bytes as a uint8 array."""
+        return (self.frames, self.channels, BYTES[self.encoding])
+
+    @property
+    def nbytes(self):
+        return self.stop - self.start
+
+    def readinto(self, buf):
+        """Reads the samples into the writable buffer buf (nbytes long) with no intermediate copy."""
+        view = memoryview(buf).cast('B')
+        with open(self.path, 'rb', buffering=0) as f:
+            f.seek(self.start)
+            done = 0
+            while done < len(view):
+                n = f.readinto(view[done:])
+                if not n:
+                    raise EOFError('%s ends inside its data chunk' % self.path)
+                done += n
+
+
+def wav_data(path):
+    """WavData of the WAV file at `path`, read from its header alone.  Handles WAVE_FORMAT_EXTENSIBLE, chunks before
+    `data` (odd sizes padded) and a data size of 0xFFFFFFFF (to the end of the file), as read_wav does.  The container
+    bit depth decides the encoding (24 valid bits in 32 is s32, as read_wav reads it), and a trailing partial frame is
+    dropped.  ValueError for a file that is not a RIFF/WAVE, NotImplementedError for an encoding read_wav lacks."""
+    with open(path, 'rb') as f:
+        with mmap.mmap(f.fileno(), 0, access=mmap.ACCESS_READ) as raw:
+            (tag, nch, sr, _, _, bits), start, stop = _wav_chunks(raw)
+    enc = _ENCODINGS.get((tag, bits))
+    if enc is None:
+        raise NotImplementedError('WAV format tag %d with %d bits' % (tag, bits))
+    if nch < 1:
+        raise ValueError('WAV header with %d channels' % nch)
+    frames = (stop - start) // (nch * BYTES[enc])
+    return WavData(path, enc, nch, sr, frames, start, start + frames * nch * BYTES[enc])
 
 
 def read_wav(path_or_file, dtype='float64', return_int16=False):

@@ -22,6 +22,9 @@ TARGET_RATE = 16000
 MIN_RATE, MAX_RATE = 8000, 192000
 MAX_CHANNELS = 8
 KAISER_BETA = 5.0
+# pcm_format of each WAV encoding (io.wav_data); the device reads u8 / s24 / s32 / f64 only through WAV files
+PCM_FORMATS = {'u8': _lib.PCM_U8, 's16': _lib.PCM_S16, 's24': _lib.PCM_S24, 's32': _lib.PCM_S32, 'f32': _lib.PCM_F32,
+               'f64': _lib.PCM_F64}
 
 
 def check_rate(rate):
@@ -170,11 +173,17 @@ def _ensure_taps(ctx, rate):
         done.add(rate)
 
 
-def to16k_multi(ctx, pcms, rate, out, out_off, stream=None):
+def to16k_multi(ctx, pcms, rate, out, out_off, stream=None, encoding=None):
     """Resamples CUDA tensors of one rate, channel count and dtype ([frames] or [frames, channels], contiguous) in one
-    launch; recording i's num_frames(len, rate) samples go to the int16 CUDA tensor `out` from out_off[i]."""
+    launch; recording i's num_frames(len, rate) samples go to the int16 CUDA tensor `out` from out_off[i].  With an
+    `encoding` (a key of PCM_FORMATS), the tensors are uint8 [frames, channels, bytes per sample]: samples as a WAV
+    stores them (io.WavData.shape)."""
     x0 = pcms[0]
-    fmt = {torch.int16: _lib.PCM_S16, torch.float32: _lib.PCM_F32}[x0.dtype]
+    if encoding is None:
+        fmt = {torch.int16: _lib.PCM_S16, torch.float32: _lib.PCM_F32}[x0.dtype]
+    else:
+        fmt = PCM_FORMATS[encoding]
+        assert x0.dtype == torch.uint8 and x0.dim() == 3
     C = channels(x0)
     assert all(p.is_cuda and p.is_contiguous() and p.dtype == x0.dtype and channels(p) == C for p in pcms)
     _ensure_taps(ctx, rate)
@@ -206,10 +215,12 @@ def window_multi(ctx, pcms, win, rate, out, stream=None):
         'iss_resample_window_multi')
 
 
-def resample_pass(ctx, pcms, rates):
+def resample_pass(ctx, pcms, rates, encodings=None):
     """16 kHz mono device views of the device recordings of one pass (what _stage_pass returns), one launch per
-    (rate, channels, dtype) group.  16 kHz mono recordings are returned as they are; the others land in one int16
-    buffer, each 16-byte aligned."""
+    (rate, channels, dtype, encoding) group.  encodings[i] is None, or the encoding of a WAV's stored bytes (see
+    to16k_multi).  16 kHz mono recordings are returned as they are; the others land in one int16 buffer, each 16-byte
+    aligned."""
+    encodings = encodings or [None] * len(pcms)
     todo = [i for i, (p, r) in enumerate(zip(pcms, rates)) if not (r == TARGET_RATE and p.dim() == 1)]
     if not todo:
         return list(pcms)
@@ -218,9 +229,9 @@ def resample_pass(ctx, pcms, rates):
     out = torch.empty(int(off[-1]), dtype=torch.int16, device=pcms[todo[0]].device)
     groups = {}
     for j, i in enumerate(todo):
-        groups.setdefault((rates[i], channels(pcms[i]), pcms[i].dtype), []).append(j)
-    for (rate, _, _), js in groups.items():
-        to16k_multi(ctx, [pcms[todo[j]] for j in js], rate, out, [off[j] for j in js])
+        groups.setdefault((rates[i], channels(pcms[i]), pcms[i].dtype, encodings[i]), []).append(j)
+    for (rate, _, _, enc), js in groups.items():
+        to16k_multi(ctx, [pcms[todo[j]] for j in js], rate, out, [off[j] for j in js], encoding=enc)
     res = list(pcms)
     for j, i in enumerate(todo):
         res[i] = out[off[j]:off[j] + n16[j]]

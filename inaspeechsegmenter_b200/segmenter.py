@@ -23,7 +23,7 @@ import torch
 
 from . import _lib, engine, models, pack, resample
 from .export_funcs import seg2csv, seg2textgrid
-from .io import media2sig16kmono
+from .io import media2sig16kmono, wav_data
 from .sidekit_mfcc import SidekitFrontEnd
 
 PATCH_W = 68
@@ -80,24 +80,31 @@ _TORCH_DTYPE = {np.dtype(np.int16): torch.int16, np.dtype(np.float32): torch.flo
 
 
 def _stage_pass(sigs, dev):
-    """Device views of the signals of one pass (numpy arrays or CUDA tensors, int16 or float32, any shape): CUDA
-    tensors are used in place, host arrays are copied into one pinned staging buffer, each 16-byte aligned (vector
-    loads in the kernels), and uploaded in one copy."""
-    host = [i for i, s in enumerate(sigs) if isinstance(s, np.ndarray)]
+    """Device views of the signals of one pass (numpy arrays or CUDA tensors, int16 or float32, any shape, or
+    io.WavData): CUDA tensors are used in place; host arrays are copied, and WAV data chunks read, into one pinned
+    staging buffer, each 16-byte aligned (vector loads in the kernels), and uploaded in one copy.  A WAV comes back as
+    its stored bytes, uint8 [frames, channels, bytes per sample]."""
+    host = [i for i, s in enumerate(sigs) if not isinstance(s, torch.Tensor)]
     pcms = list(sigs)
     if host:
         off = np.concatenate(([0], np.cumsum([(sigs[i].nbytes + 15) // 16 * 16 for i in host]))).astype(np.int64)
-        stage = np.zeros(int(off[-1]), dtype=np.uint8)
-        for k, i in enumerate(host):
-            stage[off[k]:off[k] + sigs[i].nbytes] = sigs[i].reshape(-1).view(np.uint8)
-        buf = torch.from_numpy(stage)
         try:
-            buf = buf.pin_memory()
+            buf = torch.empty(int(off[-1]), dtype=torch.uint8, pin_memory=True)
         except RuntimeError:
-            pass
+            buf = torch.empty(int(off[-1]), dtype=torch.uint8)
+        stage = buf.numpy()
+        for k, i in enumerate(host):
+            a, b = int(off[k]), int(off[k]) + sigs[i].nbytes
+            if isinstance(sigs[i], np.ndarray):
+                stage[a:b] = sigs[i].reshape(-1).view(np.uint8)
+            else:
+                sigs[i].readinto(stage[a:b])
+            stage[b:off[k + 1]] = 0
         buf = buf.to(dev, non_blocking=True)
         for k, i in enumerate(host):
-            pcms[i] = buf[off[k]:off[k] + sigs[i].nbytes].view(_TORCH_DTYPE[sigs[i].dtype]).view(sigs[i].shape)
+            v = buf[off[k]:off[k] + sigs[i].nbytes]
+            pcms[i] = v.view(_TORCH_DTYPE[sigs[i].dtype]).view(sigs[i].shape) if isinstance(sigs[i], np.ndarray) \
+                else v.view(sigs[i].shape)
     return pcms
 
 
@@ -128,7 +135,32 @@ def feats_from_signal(sig, device=0, fft_precision=_lib.FFT_FP64, ctx_name='feat
     return mspec, loge, difflen
 
 
+def _device_wav(medianame, start_sec, stop_sec, ffmpeg):
+    """The io.WavData of a whole file read without ffmpeg that is a WAV but not 16 kHz mono: the device decodes and
+    resamples it (_wav_to16k).  None for every other call, which keeps media2sig16kmono's path and errors."""
+    if ffmpeg is not None or start_sec is not None or stop_sec is not None:
+        return None
+    try:
+        wav = wav_data(medianame)
+    except Exception:           # not a readable WAV: media2sig16kmono reports it
+        return None
+    return None if (wav.rate == resample.TARGET_RATE and wav.channels == 1) else wav
+
+
+def _wav_to16k(ctx, wav):
+    """A WAV's data chunk read into the pinned staging buffer, uploaded once and resampled to 16 kHz mono int16 on
+    the device: what segment_signal(x, sample_rate=wav.rate) feeds the front ends, for x the file's samples."""
+    resample.check_rate(wav.rate)
+    if not 1 <= wav.channels <= resample.MAX_CHANNELS:
+        raise ValueError('%d channels: 1 to %d are supported' % (wav.channels, resample.MAX_CHANNELS))
+    return resample.resample_pass(ctx, _stage_pass([wav], ctx.device), [wav.rate], [wav.encoding])[0]
+
+
 def _media2feats(medianame, start_sec, stop_sec, ffmpeg, device=0, fft_precision=_lib.FFT_FP64, ctx_name='feat'):
+    wav = _device_wav(medianame, start_sec, stop_sec, ffmpeg)
+    if wav is not None:
+        return feats_from_signal(_wav_to16k(_get_ctx(ctx_name, device), wav), device, fft_precision, ctx_name,
+                                 medianame)
     sig = media2sig16kmono(medianame, start_sec, stop_sec, ffmpeg, 'float32', return_int16=True)
     if sig.ndim > 1:
         raise ValueError('expected a mono signal, got shape %r' % (sig.shape,))

@@ -419,12 +419,15 @@ class VoiceFemininityScoring:
         or channel count, what ``Segmenter.segment_signal`` resamples (then resampled to 16 kHz int16 on the device)."""
         from . import resample
         if not resample.is_native(sig, sample_rate):
-            sig = pcm = resample.to16k(self.ctx, sig, sample_rate)
-        else:
-            sig = np.asarray(sig)
-            sig = sig.reshape(-1) if sig.ndim == 2 else sig
-            sig = sig if sig.dtype in (np.int16, np.float32) else sig.astype(np.float32)
-            pcm = None
+            return self._score_16k(resample.to16k(self.ctx, sig, sample_rate), basename)
+        sig = np.asarray(sig)
+        sig = sig.reshape(-1) if sig.ndim == 2 else sig
+        sig = sig if sig.dtype in (np.int16, np.float32) else sig.astype(np.float32)
+        return self._score_16k(sig, basename)
+
+    def _score_16k(self, sig, basename):
+        """score_signal on 16 kHz mono: a host array, or the int16 CUDA tensor of a resampled recording."""
+        pcm = sig if isinstance(sig, torch.Tensor) else None
         duration = len(sig) / SR
         vad_seg = self.vad.segment_signal(sig)
         speech = [(b, e) for lab, b, e in vad_seg if lab == 'speech']
@@ -516,6 +519,10 @@ class VoiceFemininityScoring:
     def __call__(self, fpath):
         """Voice femininity score of a media file (vbx_segmenter.py:147-202)."""
         from .io import media2sig16kmono
+        from .segmenter import _device_wav, _wav_to16k
         basename = os.path.splitext(os.path.basename(fpath))[0]
+        wav = _device_wav(fpath, None, None, self.ffmpeg)
+        if wav is not None:         # a WAV that is not 16 kHz mono, without ffmpeg: decoded on the device
+            return self._score_16k(_wav_to16k(self.ctx, wav), basename)
         sig = media2sig16kmono(fpath, ffmpeg=self.ffmpeg, dtype='float32', return_int16=True)
         return self.score_signal(sig, basename)

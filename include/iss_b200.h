@@ -39,7 +39,7 @@ typedef struct iss_mlp iss_mlp;
 
 /* ---- library / context ------------------------------------------------- */
 
-#define ISS_ABI_VERSION 8
+#define ISS_ABI_VERSION 9
 int         iss_version(void);               /* == ISS_ABI_VERSION of the header the library was built from */
 const char *iss_last_error(void);
 /* Creates a context bound to CUDA device `device` (one per host thread that
@@ -69,6 +69,11 @@ int iss_get_gemm_mode(void);
 
 #define ISS_PCM_F32 0   /* float32 samples in [-1, 1) (what soundfile returns, io.py:51) */
 #define ISS_PCM_S16 1   /* int16 PCM; converted as s / 32768.0f, exactly what soundfile does */
+/* WAV encodings only the resampler reads (ISS_ERR_INVALID everywhere else), with their float64 value: */
+#define ISS_PCM_U8  2   /* unsigned 8-bit, (s - 128) / 128 */
+#define ISS_PCM_S24 3   /* signed 24-bit, 3 bytes little-endian, packed; s / 2^23 */
+#define ISS_PCM_S32 4   /* signed 32-bit, s / 2^31 */
+#define ISS_PCM_F64 5   /* IEEE float64, as is */
 
 #define ISS_FFT_FP32 0  /* single-precision FFT (fast) */
 #define ISS_FFT_FP64 1  /* double-precision window + FFT, power rounded to f32: the
@@ -334,9 +339,10 @@ int iss_dither_mt19937_multi(iss_ctx *ctx, int n_rec, const int64_t *h_rec, uint
 /* ---- Resampling to 16 kHz mono -----------------------------------------------
  * No reference counterpart: the reference has ffmpeg decode with `-ar 16000 -ac 1`
  * (io.py:37-55).  This is NOT ffmpeg's resampler.  A recording of n frames of C
- * interleaved channels at integer rate R (8000 <= R <= 192000, 1 <= C <= 8, int16 or
- * float32 samples laid out [frames][channels]) becomes int16 16 kHz mono PCM:
- *   x[m]   = mean of the C samples of frame m in float64 (int16 s as s / 32768.0),
+ * interleaved channels at integer rate R (8000 <= R <= 192000, 1 <= C <= 8, samples of
+ * any ISS_PCM_* format laid out [frames][channels]) becomes int16 16 kHz mono PCM:
+ *   x[m]   = mean of the C samples of frame m in float64 (each as its format's value:
+ *            int16 s as s / 32768.0, float32 as is, the WAV encodings as listed above),
  *   y      = scipy.signal.resample_poly(x, up, down) with up = 16000 / g, down = R / g,
  *            g = gcd(16000, R) (scipy's default Kaiser(5.0) design, zero padding),
  *   out[k] = clip(rint(y[k] * 32768), -32768, 32767)  (round half to even),
@@ -356,7 +362,8 @@ int iss_resample_release_taps(iss_ctx *ctx, int rate);
  * r is h_pcm[r] (a DEVICE pointer held in a host array) with h_n_frames[r] frames; its
  * iss_resample_num_frames(h_n_frames[r], rate) int16 outputs go to d_out[h_out_off[r] ..].
  * Any pointer alignment of the sample type works (16-byte aligned recordings are read
- * with vector loads).  ISS_ERR_STATE if no taps were uploaded for `rate`. */
+ * with vector loads; packed 24-bit recordings at any byte address).  No load reads a byte
+ * outside a recording's frames.  ISS_ERR_STATE if no taps were uploaded for `rate`. */
 int iss_resample_to16k_multi(iss_ctx *ctx, int n_rec, const void *const *h_pcm, const int64_t *h_n_frames,
                              int channels, int rate, int pcm_format, int16_t *d_out, const int64_t *h_out_off,
                              void *stream);
