@@ -12,8 +12,9 @@
 //
 // Layout: one CTA owns a tile of consecutive outputs of one record (tiles start at the record's first output k_first).
 // It stages the raw samples of the tile's input span in shared memory with 16-byte loads (scalar loads when the
-// record's base pointer is not 16-byte aligned; packed 24-bit samples are staged as bytes and sign-extended in the
-// downmix), downmixes them there into float64, then each thread evaluates
+// record's base pointer is not 16-byte aligned, byte loads when it is not even aligned to its samples, as a WAV's
+// stored bytes may lie at any address; packed 24-bit samples are staged as bytes and sign-extended in the downmix),
+// downmixes them there into float64, then each thread evaluates
 // its outputs as float64 FMA chains in ascending frame order.  No atomics, and no value depends on the tiling.
 //
 // Windows (live streams): a record's buffer holds frames [f_base, n_known) of its stream, and it computes outputs
@@ -53,7 +54,7 @@ struct RsRec {
     int64_t n_out;
     int64_t out_off;                // int16 element of output k_first
     int64_t tile_off;               // first tile (global block index); entry n_rec holds the total
-    int vec_ok;                     // pcm is 16-byte aligned
+    int align;                      // pcm is 16-byte aligned (2), aligned to its Unit (1), or neither (0)
 };
 
 // A stored sample is UNITS consecutive Units (what the staging loads: bytes for packed 24-bit) in record order.
@@ -109,7 +110,7 @@ resample_kernel(const RsRec *__restrict__ recs, int n_rec, const Phase *__restri
     int64_t rb = 0;                                              // raw[i] holds unit rb + i of pcm
     if (g_lo < g_hi) {
         const int64_t e_lo = (g_lo - fb) * channels * UNITS, e_hi = (g_hi - fb) * channels * UNITS;
-        if (rec.vec_ok) {
+        if (rec.align == 2) {
             rb = e_lo & ~(int64_t)(VEC - 1);
             const int64_t v_hi = e_hi & ~(int64_t)(VEC - 1);
             const int nv = (int)((v_hi - rb) / VEC);
@@ -117,9 +118,15 @@ resample_kernel(const RsRec *__restrict__ recs, int n_rec, const Phase *__restri
             int4 *dst = reinterpret_cast<int4 *>(raw);
             for (int i = tid; i < nv; i += RS_THREADS) dst[i] = __ldg(src + i);
             for (int64_t e = max(v_hi, rb) + tid; e < e_hi; e += RS_THREADS) raw[e - rb] = pcm[e];
-        } else {
+        } else if (sizeof(Unit) == 1 || rec.align == 1) {
             rb = e_lo;
             for (int64_t e = e_lo + tid; e < e_hi; e += RS_THREADS) raw[e - rb] = pcm[e];
+        } else {
+            rb = e_lo;
+            const unsigned char *src = reinterpret_cast<const unsigned char *>(pcm + e_lo);
+            unsigned char *dst = reinterpret_cast<unsigned char *>(raw);
+            const int64_t nb = (e_hi - e_lo) * (int64_t)sizeof(Unit);
+            for (int64_t i = tid; i < nb; i += RS_THREADS) dst[i] = src[i];
         }
     }
     __syncthreads();
@@ -331,13 +338,15 @@ static int run_records(iss_ctx *ctx, const char *fn, const ResampleTable &t, std
     int tile, span_cap;
     size_t smem;
     tile_for(t, channels, sample_bytes(pcm_format), &tile, &span_cap, &smem);
+    const uintptr_t unit = pcm_format == ISS_PCM_S24 ? 1 : (uintptr_t)sample_bytes(pcm_format);     // bytes of a Unit
     ISS_REQUIRE(smem <= (size_t)RS_SMEM_BUDGET, ISS_ERR_INVALID, "%s: staged span of %zu bytes over the budget", fn, smem);
     const int n_rec = (int)recs.size() - 1;
     int64_t ntiles = 0;
     for (int i = 0; i < n_rec; ++i) {
         RsRec &r = recs[i];
         r.tile_off = ntiles;
-        r.vec_ok = ((reinterpret_cast<uintptr_t>(r.pcm) & 15) == 0) ? 1 : 0;
+        const uintptr_t a = reinterpret_cast<uintptr_t>(r.pcm);
+        r.align = (a & 15) == 0 ? 2 : (a % unit == 0 ? 1 : 0);
         ntiles += (r.n_out + tile - 1) / tile;
     }
     recs[n_rec] = RsRec{nullptr, 0, 0, 0, 0, 0, ntiles, 0};

@@ -7,6 +7,7 @@ import pytest
 
 from conftest import synth_audio
 from oracle import resample_ref as rr
+from resample_fixtures import reference
 
 pytestmark = pytest.mark.gpu
 
@@ -43,7 +44,7 @@ def _recording(rate, n, C, fmt, seed):
 
 
 def _check(got, x, rate, what):
-    q, tie, _, _ = rr.reference(x, rate)
+    q, tie, _, _ = reference(x, rate)
     got = got.cpu().numpy() if isinstance(got, torch.Tensor) else got
     assert got.shape == q.shape, what
     bad = (got != q) & ~tie
@@ -173,7 +174,7 @@ def test_segment_signal_resampled_equals_reference_pcm(rt, synth_models):
     with warnings.catch_warnings():
         warnings.simplefilter('ignore')
         for x, rate in ((synth_audio(60, sr=48000), 48000), (_stereo(60, 44100, 31), 44100)):
-            q, tie, _, _ = rr.reference(x, rate)
+            q, tie, _, _ = reference(x, rate)
             assert not tie.any()
             got = seg.segment_signal(x, sample_rate=rate)
             assert got == seg.segment_signal(q)
@@ -247,7 +248,7 @@ def test_score_signal_and_signals_resampled(rt, synth_models):
     from test_vfs_pack_gpu import vfs_models
     vfs = vb.VoiceFemininityScoring(ffmpeg=None, models=vfs_models(synth_models))
     x48 = _stereo(30, 48000, 70)
-    q, tie, _, _ = rr.reference(x48, 48000)
+    q, tie, _, _ = reference(x48, 48000)
     assert not tie.any()
 
     def score(fn):

@@ -8,7 +8,7 @@ import numpy as np
 import pytest
 
 from conftest import synth_audio
-from oracle import resample_ref as rr
+from resample_fixtures import reference
 from wav_fixtures import decode, encode, fixtures, write_wav
 
 pytestmark = pytest.mark.gpu
@@ -36,7 +36,7 @@ def _stored(w):
 
 
 def _check(got, x, rate, what):
-    q, tie, _, _ = rr.reference(x, rate)
+    q, tie, _, _ = reference(x, rate)
     got = got.cpu().numpy() if isinstance(got, torch.Tensor) else got
     assert got.shape == q.shape, what
     assert not tie.any(), (what, int(tie.sum()))
@@ -120,7 +120,7 @@ def _expected_pcm(rt, path):
     s16, s24, f32), else the oracle's 16 kHz int16 output (s32, f64)."""
     w = rt['io'].wav_data(path)
     if w.encoding in ('s32', 'f64'):
-        q, tie, _, _ = rr.reference(decode(_stored(w), w.encoding, w.channels), w.rate)
+        q, tie, _, _ = reference(decode(_stored(w), w.encoding, w.channels), w.rate)
         assert not tie.any()
         return q, 16000
     x, sr = rt['io'].read_wav(path, 'float32')

@@ -49,17 +49,17 @@ def decode(raw, encoding, channels):
 
 
 def write_wav(path, data, encoding, channels, rate, extensible=False, valid_bits=None, pre_chunks=(),
-              unknown_size=False, tail=b''):
+              unknown_size=False, tail=b'', channel_mask=0):
     """Writes a RIFF/WAVE file whose data chunk holds the bytes `data` (then `tail`, e.g. a partial frame).
-    extensible: WAVE_FORMAT_EXTENSIBLE with the sub-format of `encoding` and valid_bits (the container's by default);
-    pre_chunks: (id, body) chunks written between fmt and data, odd bodies padded; unknown_size: data size 0xFFFFFFFF
-    and RIFF size 0xFFFFFFFF, as ffmpeg writes to a pipe."""
+    extensible: WAVE_FORMAT_EXTENSIBLE with the sub-format of `encoding`, valid_bits (the container's by default) and
+    channel_mask; pre_chunks: (id, body) chunks written between fmt and data, odd bodies padded; unknown_size: data
+    size 0xFFFFFFFF and RIFF size 0xFFFFFFFF, as ffmpeg writes to a pipe."""
     tag, bits = _TAG_BITS[encoding]
     block = channels * bits // 8
     fmt = struct.pack('<HHIIHH', 0xFFFE if extensible else tag, channels, rate, rate * block, block, bits)
     if extensible:
         guid_tail = b'\x00\x00\x00\x00\x10\x00\x80\x00\x00\xaa\x00\x38\x9b\x71'
-        fmt += struct.pack('<HHI', 22, valid_bits or bits, 0) + struct.pack('<H', tag) + guid_tail
+        fmt += struct.pack('<HHI', 22, valid_bits or bits, channel_mask) + struct.pack('<H', tag) + guid_tail
     body = b'WAVE' + b'fmt ' + struct.pack('<I', len(fmt)) + fmt
     for cid, chunk in pre_chunks:
         body += cid + struct.pack('<I', len(chunk)) + chunk + (b'\x00' if len(chunk) & 1 else b'')
@@ -107,4 +107,26 @@ def fixtures(directory, frames=3001):
     for name, (kw, enc, C) in forms.items():
         path = os.path.join(directory, name + '.wav')
         out[name] = (write_wav(path, encode(x[:, :C], enc), enc, C, 48000, **kw), enc, C, 48000)
+    return out
+
+
+# dwChannelMask of WAVE_FORMAT_EXTENSIBLE for each channel count over 2: front left / right / centre, LFE, back
+# left / right, side left / right (3.0, quad, 5.0, 5.1, 6.1, 7.1)
+CHANNEL_MASKS = {3: 0x7, 4: 0x33, 5: 0x37, 6: 0x3F, 7: 0x70F, 8: 0x63F}
+DOMAIN_CHANNELS = (3, 4, 5, 7, 8)
+DOMAIN_RATES = (11025, 32000, 88200, 96000, 176400, 191999)
+
+
+def domain_fixtures(directory, encodings=ENCODINGS, channels=DOMAIN_CHANNELS, rates=DOMAIN_RATES, frames=2001):
+    """{name: (path, encoding, channels, rate)}: every encoding x channel count x rate given, as a multichannel file
+    is written: WAVE_FORMAT_EXTENSIBLE with the channel mask of its layout over 2 channels, the plain header below."""
+    out = {}
+    for enc in encodings:
+        for C in channels:
+            for rate in rates:
+                name = '%s_%dch_%d' % (enc, C, rate)
+                x = signal(frames, C, rate, seed=1000 + len(out))
+                kw = dict(extensible=True, channel_mask=CHANNEL_MASKS[C]) if C > 2 else {}
+                out[name] = (write_wav(os.path.join(directory, name + '.wav'), encode(x, enc), enc, C, rate, **kw),
+                             enc, C, rate)
     return out
